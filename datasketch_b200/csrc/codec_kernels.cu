@@ -7,7 +7,7 @@
 //                            bulk store of the finished tile (cp.async.bulk.global.shared::cta).
 //  band_keys_be            : [N,K] u32 -> [N, b, 8r] bytes: each band's r values as big-endian
 //                            u64 (the dict keys MinHashLSH._H builds, lsh.py:344, :537-538).
-//  band_fingerprints       : [N,K] u32 -> [N, b] u64 mix of each band's r-tuple (GPU bucketing;
+//  band_fingerprints       : [N,K] u32 -> [N, b] u64 bucket key of each band's r-tuple (GPU bucketing;
 //                            candidates are verified on the exact r-tuple, see lsh_kernels.cu).
 #include <algorithm>
 
@@ -189,23 +189,15 @@ __global__ void __launch_bounds__(256) band_keys_be_kernel(const uint32_t *__res
     }
 }
 
-// 64-bit mix of a band's r-tuple (xor-multiply chain + final avalanche); equal tuples <=> equal
-// fingerprints up to 2^-64 collisions, which the LSH kernels resolve by comparing the tuples.
-__device__ __forceinline__ uint64_t mix64(uint64_t h) {
-    h ^= h >> 32; h *= 0xD6E8FEB86659FD93ull; h ^= h >> 32; h *= 0xD6E8FEB86659FD93ull; h ^= h >> 32;
-    return h;
-}
-
+// The LSH index's bucket key of each band (band_fp, dsk_common.cuh: the tables' empty key remapped included); equal
+// tuples <=> equal fingerprints up to 2^-64 collisions, which the LSH kernels resolve by comparing the tuples.
 __global__ void __launch_bounds__(256) band_fingerprint_kernel(const uint32_t *__restrict__ sig, int64_t n, int k,
                                                                int b, int r, uint64_t *__restrict__ out) {
     const int64_t total = n * b, stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += stride) {
         const int64_t i = e / b;
         const int band = (int)(e - i * b);
-        const uint32_t *v = sig + i * k + (int64_t)band * r;
-        uint64_t h = 0x9E3779B97F4A7C15ull ^ (uint64_t)band;
-        for (int q = 0; q < r; ++q) h = (h ^ v[q]) * 0xFF51AFD7ED558CCDull + 0x2545F4914F6CDD1Dull;
-        out[e] = mix64(h);
+        out[e] = band_fp(sig + i * k + (int64_t)band * r, r, band);
     }
 }
 

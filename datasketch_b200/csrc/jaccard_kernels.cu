@@ -50,6 +50,7 @@ __global__ void __launch_bounds__(256) jaccard_pairs_kernel(const uint32_t *__re
 // sorted list in shared memory (ties keep the lower database index because tiles arrive in index
 // order and insertion requires a strictly larger count than the k-th entry ... or an unfilled slot).
 constexpr int kTQ = 64, kTD = 128, kKc = 32, kTopThreads = 128, kMaxTopK = 32;
+constexpr size_t kMaxSmemPerBlock = 232448;   // the dynamic shared memory one sm_90 block can opt into (227 KB)
 
 struct TopkParams {
     const uint32_t *q;    // [nq, k]
@@ -156,6 +157,132 @@ __global__ void __launch_bounds__(kTopThreads) jaccard_topk_kernel(const TopkPar
                             int32_t *tc = top_cnt + ql * kMaxTopK;
                             int64_t *ti = top_idx + ql * kMaxTopK;
                             // position: after every entry with count > c, or count == c and lower index
+                            int pos = topk;
+                            for (int s = 0; s < topk; ++s) {
+                                const int32_t sc = tc[s];
+                                if (sc < c || (sc == c && (ti[s] < 0 || ti[s] > drow))) { pos = s; break; }
+                            }
+                            if (pos < topk) {
+                                for (int s = topk - 1; s > pos; --s) { tc[s] = tc[s - 1]; ti[s] = ti[s - 1]; }
+                                tc[pos] = c; ti[pos] = drow;
+                                kidx[ql] = ti[topk - 1];
+                                thr[ql] = (ti[topk - 1] < 0) ? -1 : tc[topk - 1];
+                            }
+                            __threadfence_block();
+                            atomicExch(&lock[ql], 0);
+                            done = true;
+                        }
+                    }
+                }
+            }
+        }
+        __syncthreads();
+        for (int e = tid; e < kTQ * topk; e += kTopThreads) {
+            const int r = e / topk, s = e - r * topk;
+            if (q0 + r < p.nq) {
+                p.out_cnt[(q0 + r) * topk + s] = top_cnt[r * kMaxTopK + s];
+                p.out_idx[(q0 + r) * topk + s] = top_idx[r * kMaxTopK + s];
+            }
+        }
+    }
+}
+
+// The same lists for K whose resident query tile does not fit in a block's shared memory (jaccard_topk_smem(K) > 227 KB,
+// i.e. K > 736): the query tile is staged 32 positions at a time next to the database chunk, so each database tile
+// re-reads it (from L2) instead of keeping it resident.  Counting and list updates are those of jaccard_topk_kernel.
+__global__ void __launch_bounds__(kTopThreads) jaccard_topk_wide_kernel(const TopkParams p) {
+    DSK_DYNAMIC_SMEM_T(uint32_t, sm, 16);
+    const int K = p.k;
+    const int kpad = (K + kKc - 1) / kKc * kKc;
+    uint32_t *sQ = sm;                              // [kKc][kTQ]
+    uint32_t *sD = sQ + kKc * kTQ;                  // [kKc][kTD]
+    int32_t *top_cnt = reinterpret_cast<int32_t *>(sD + kKc * kTD);   // [kTQ][topk]
+    int64_t *top_idx = reinterpret_cast<int64_t *>(top_cnt + kTQ * kMaxTopK);  // [kTQ][topk]
+    int *lock = reinterpret_cast<int *>(top_idx + kTQ * kMaxTopK);    // [kTQ]
+    volatile int32_t *thr = reinterpret_cast<volatile int32_t *>(lock + kTQ);  // [kTQ] k-th best count, -1 while unfilled
+    volatile int64_t *kidx = reinterpret_cast<volatile int64_t *>(const_cast<int32_t *>(thr) + kTQ);  // [kTQ] its index
+
+    const int tid = threadIdx.x;
+    const int qg = tid >> 4, dg = tid & 15;         // 8 query groups x 16 database groups
+    const int topk = p.topk;
+
+    for (int64_t qt = blockIdx.x; qt * kTQ < p.nq; qt += gridDim.x) {
+        const int64_t q0 = qt * kTQ;
+        __syncthreads();
+        for (int i = tid; i < kTQ * kMaxTopK; i += kTopThreads) { top_cnt[i] = -1; top_idx[i] = -1; }
+        for (int i = tid; i < kTQ; i += kTopThreads) { lock[i] = 0; thr[i] = -1; kidx[i] = -1; }
+
+        for (int64_t d0 = 0; d0 < p.n; d0 += kTD) {
+            int cnt[8][8];
+#pragma unroll
+            for (int a = 0; a < 8; ++a)
+#pragma unroll
+                for (int b = 0; b < 8; ++b) cnt[a][b] = 0;
+            for (int c0 = 0; c0 < kpad; c0 += kKc) {
+                __syncthreads();
+                // query chunk [kKc positions][kTQ rows], transposed; positions / rows beyond the data never match
+                for (int e = tid; e < kTQ * kKc; e += kTopThreads) {
+                    const int r = e / kKc, c = e - r * kKc;
+                    uint32_t v = 0x51EDu + (uint32_t)(c0 + c);    // the db side fills with ~filler
+                    if (q0 + r < p.nq && c0 + c < K) v = __ldg(p.q + (q0 + r) * (int64_t)K + c0 + c);
+                    sQ[c * kTQ + r] = v;
+                }
+                // database chunk [kTD rows][kKc positions], transposed: each task = (row, 8 positions)
+                for (int task = tid; task < kTD * (kKc / 8); task += kTopThreads) {
+                    const int r = task % kTD, seg = task / kTD;
+                    const int64_t row = d0 + r;
+                    const int cb = c0 + seg * 8;
+                    uint32_t v[8];
+                    if (row < p.n && (K & 3) == 0 && cb + 8 <= K) {
+                        const uint4 x = __ldg(reinterpret_cast<const uint4 *>(p.db + row * (int64_t)K + cb));
+                        const uint4 y = __ldg(reinterpret_cast<const uint4 *>(p.db + row * (int64_t)K + cb + 4));
+                        v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w; v[4] = y.x; v[5] = y.y; v[6] = y.z; v[7] = y.w;
+                    } else {
+#pragma unroll
+                        for (int u = 0; u < 8; ++u) {
+                            v[u] = ~(0x51EDu + (uint32_t)(cb + u));
+                            if (row < p.n && cb + u < K) v[u] = __ldg(p.db + row * (int64_t)K + cb + u);
+                        }
+                    }
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) sD[(seg * 8 + u) * kTD + r] = v[u];
+                }
+                __syncthreads();
+#pragma unroll 4
+                for (int cc = 0; cc < kKc; ++cc) {
+                    const uint4 qa = *reinterpret_cast<const uint4 *>(sQ + cc * kTQ + qg * 8);
+                    const uint4 qb = *reinterpret_cast<const uint4 *>(sQ + cc * kTQ + qg * 8 + 4);
+                    const uint4 da = *reinterpret_cast<const uint4 *>(sD + cc * kTD + dg * 8);
+                    const uint4 db = *reinterpret_cast<const uint4 *>(sD + cc * kTD + dg * 8 + 4);
+                    const uint32_t qv[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
+                    const uint32_t dv[8] = {da.x, da.y, da.z, da.w, db.x, db.y, db.z, db.w};
+#pragma unroll
+                    for (int a = 0; a < 8; ++a)
+#pragma unroll
+                        for (int b = 0; b < 8; ++b) cnt[a][b] += (qv[a] == dv[b]);
+                }
+            }
+            // fold this tile's counts into the per-query sorted lists
+#pragma unroll
+            for (int a = 0; a < 8; ++a) {
+                const int ql = qg * 8 + a;
+                const int64_t qrow = q0 + ql;
+                if (qrow >= p.nq) continue;
+#pragma unroll
+                for (int b = 0; b < 8; ++b) {
+                    const int64_t drow = d0 + dg * 8 + b;
+                    if (drow >= p.n) continue;
+                    if (p.self_base >= 0 && drow == p.self_base + qrow) continue;
+                    const int c = cnt[a][b];
+                    {
+                        const int32_t t = thr[ql];
+                        if (c < t || (c == t && drow > kidx[ql])) continue;
+                    }
+                    bool done = false;
+                    while (!done) {
+                        if (atomicCAS(&lock[ql], 0, 1) == 0) {
+                            int32_t *tc = top_cnt + ql * kMaxTopK;
+                            int64_t *ti = top_idx + ql * kMaxTopK;
                             int pos = topk;
                             for (int s = 0; s < topk; ++s) {
                                 const int32_t sc = tc[s];
@@ -372,10 +499,18 @@ __global__ void __launch_bounds__(kTopThreads) jaccard_topk_pf_kernel(const Topk
     }
 }
 
-// workspace of the prefilter path: the bit planes of both matrices (0 = the path does not apply: K < 32 or K > 512)
+// shared memory of jaccard_topk_pf_kernel: both tiles' bit planes, the lists, the candidate queue
+static size_t jaccard_topk_pf_smem(int words) {
+    return (size_t)kPfB * words * (kTQ + kTD) * 4 + (size_t)kTQ * kMaxTopK * (4 + 8) + (size_t)kTQ * 16 + 16 +
+           (size_t)kTQ * kTD * 2;
+}
+
+// workspace of the prefilter path: the bit planes of both matrices (0 = the path does not apply: K < 32, or K > 480,
+// where the bit planes of a tile pair no longer fit in one block's shared memory)
 size_t jaccard_topk_workspace_bytes(int64_t nq, int64_t n, int k) {
     if (k < 32 || k > 512 || n < 4 * kTD) return 0;
     const int words = (k + 31) / 32;
+    if (jaccard_topk_pf_smem(words) > kMaxSmemPerBlock) return 0;
     const size_t qt = (size_t)((nq + kTQ - 1) / kTQ), dt = (size_t)((n + kTD - 1) / kTD);
     return (qt * kTQ + dt * kTD) * (size_t)kPfB * words * sizeof(uint32_t);
 }
@@ -394,8 +529,7 @@ cudaError_t launch_jaccard_topk_pf(const uint32_t *q, int64_t nq, const uint32_t
     TopkPfParams p;
     p.q = q; p.db = db; p.qpl = qpl; p.dpl = dpl; p.nq = nq; p.n = n; p.k = k; p.words = words; p.topk = topk;
     p.self_base = self_base; p.out_cnt = out_cnt; p.out_idx = out_idx;
-    const size_t smem = (size_t)kPfB * words * (kTQ + kTD) * 4 + (size_t)kTQ * kMaxTopK * (4 + 8) + (size_t)kTQ * 16 + 16 +
-                        (size_t)kTQ * kTD * 2;
+    const size_t smem = jaccard_topk_pf_smem(words);
     cudaError_t e = cudaFuncSetAttribute(jaccard_topk_pf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     int64_t grid = (nq + kTQ - 1) / kTQ;
@@ -415,11 +549,18 @@ cudaError_t launch_jaccard_topk(const uint32_t *q, int64_t nq, const uint32_t *d
     TopkParams p;
     p.q = q; p.db = db; p.nq = nq; p.n = n; p.k = k; p.topk = topk; p.self_base = self_base;
     p.out_cnt = out_cnt; p.out_idx = out_idx;
-    const size_t smem = jaccard_topk_smem(k);
-    cudaError_t e = cudaFuncSetAttribute(jaccard_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
     int64_t grid = (nq + kTQ - 1) / kTQ;
     if (grid > (int64_t)sm_count * 3) grid = (int64_t)sm_count * 3;
+    const size_t smem = jaccard_topk_smem(k);
+    if (smem > kMaxSmemPerBlock) {   // K > 736: the query tile is staged chunk by chunk
+        const size_t wsmem = (size_t)kKc * (kTQ + kTD) * 4 + (size_t)kTQ * kMaxTopK * (4 + 8) + (size_t)kTQ * 16;
+        cudaError_t e = cudaFuncSetAttribute(jaccard_topk_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem);
+        if (e != cudaSuccess) return e;
+        DSK_LAUNCH(jaccard_topk_wide_kernel, (unsigned)grid, kTopThreads, wsmem, s, p);
+        return cudaGetLastError();
+    }
+    cudaError_t e = cudaFuncSetAttribute(jaccard_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
     DSK_LAUNCH(jaccard_topk_kernel, (unsigned)grid, kTopThreads, smem, s, p);
     return cudaGetLastError();
 }

@@ -250,7 +250,8 @@ DSK_API int dsk_jaccard_pairs(const uint32_t *d_sig, int64_t n_rows, int num_per
 DSK_API int dsk_jaccard_topk(const uint32_t *d_q, int64_t nq, const uint32_t *d_db, int64_t n, int num_perm, int topk,
                              int64_t self_base, int32_t *d_cnt, int64_t *d_idx, void *stream);
 /* Same result, ~3x fewer ALU ops: with a caller-provided workspace (16-byte aligned, >= dsk_jaccard_topk_workspace_size()
- * bytes -- 0 means the prefilter does not apply and the call behaves like dsk_jaccard_topk) both matrices are first reduced
+ * bytes -- 0 means the prefilter does not apply (num_perm < 32 or > 480, where a tile pair's planes exceed one block's
+ * shared memory, or n < 512) and the call behaves like dsk_jaccard_topk) both matrices are first reduced
  * to bit-sliced 16-bit fingerprints; a pair reaches the exact count only if the fingerprint agreement -- an upper bound of
  * the number of equal positions -- could still enter the query's list.  Lists are identical to dsk_jaccard_topk's. */
 DSK_API size_t dsk_jaccard_topk_workspace_size(int64_t nq, int64_t n, int num_perm);

@@ -26,12 +26,19 @@
 
 typedef int cudaError_t;
 typedef void *cudaStream_t;
-enum { cudaSuccess = 0 };
+enum { cudaSuccess = 0, cudaErrorInvalidValue = 1, cudaErrorMemoryAllocation = 2, cudaErrorInsufficientDriver = 35,
+       cudaErrorNoDevice = 100 };
 enum { cudaFuncAttributeMaxDynamicSharedMemorySize = 8 };
 static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 static inline cudaError_t cudaMemsetAsync(void *p, int v, size_t n, cudaStream_t) { memset(p, v, n); return cudaSuccess; }
+// sm_90 grants one block at most 227 KB of shared memory (232,448 bytes); the runtime refuses a larger opt-in
+constexpr int kEmuMaxSharedPerBlockOptin = 232448;
 template <typename F>
-static inline cudaError_t cudaFuncSetAttribute(F, int, int) { return cudaSuccess; }
+static inline cudaError_t cudaFuncSetAttribute(F, int attr, int value) {
+    if (attr == cudaFuncAttributeMaxDynamicSharedMemorySize && (value < 0 || value > kEmuMaxSharedPerBlockOptin))
+        return cudaErrorInvalidValue;
+    return cudaSuccess;
+}
 
 struct uint3e { unsigned x, y, z; };
 struct uint2 { uint32_t x, y; };
@@ -99,7 +106,6 @@ static inline unsigned long long atomicExch(unsigned long long *p, unsigned long
 static inline void __threadfence_block() { __atomic_thread_fence(__ATOMIC_SEQ_CST); }
 
 // ---- CUDA runtime, synchronous and on host memory: "device" pointers are host pointers, one fake device with two SMs
-enum { cudaErrorInvalidValue = 1, cudaErrorMemoryAllocation = 2, cudaErrorInsufficientDriver = 35, cudaErrorNoDevice = 100 };
 enum { cudaStreamNonBlocking = 1 };
 struct cudaDeviceProp { int multiProcessorCount, major, minor; size_t totalGlobalMem; char name[64]; };
 static inline const char *cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : "emulated CUDA error"; }
