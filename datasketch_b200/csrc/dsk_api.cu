@@ -821,6 +821,66 @@ int dsk_exclusive_scan(const int64_t *d_in, int64_t n, int64_t *d_out, int64_t *
     return DSK_OK;
 }
 
+static int check_self_join(const char *who, const dsk_lsh *ix, int min_count) {
+    if (!ix) {
+        set_error("%s: null handle", who);
+        return DSK_ERR_INVALID;
+    }
+    if (min_count < 0 || min_count > ix->dev.k) {
+        set_error("%s: min_count must be in [0, num_perm=%d] (got %d)", who, ix->dev.k, min_count);
+        return DSK_ERR_INVALID;
+    }
+    return DSK_OK;
+}
+
+int dsk_lsh_pairs_count(const dsk_lsh *ix, int min_count, int64_t *d_counts, void *stream) {
+    int rc = check_self_join("dsk_lsh_pairs_count", ix, min_count);
+    if (rc) return rc;
+    if (ix->n_docs > 0 && !d_counts) {
+        set_error("dsk_lsh_pairs_count: null buffer");
+        return DSK_ERR_INVALID;
+    }
+    DevInfo *dev;
+    rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->n_docs, min_count, d_counts, nullptr, nullptr, nullptr, dev->sm_count,
+                              (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_lsh_pairs_fill(const dsk_lsh *ix, int min_count, const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq,
+                       void *stream) {
+    int rc = check_self_join("dsk_lsh_pairs_fill", ix, min_count);
+    if (rc) return rc;
+    if (ix->n_docs > 0 && (!d_ptr || !d_idx || !d_eq)) {
+        set_error("dsk_lsh_pairs_fill: null buffer");
+        return DSK_ERR_INVALID;
+    }
+    DevInfo *dev;
+    rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->n_docs, min_count, nullptr, d_ptr, d_idx, d_eq, dev->sm_count,
+                              (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_lsh_clusters(const dsk_lsh *ix, int min_count, int32_t *d_labels, void *stream) {
+    int rc = check_self_join("dsk_lsh_clusters", ix, min_count);
+    if (rc) return rc;
+    if (ix->n_docs > 0 && !d_labels) {
+        set_error("dsk_lsh_clusters: null buffer");
+        return DSK_ERR_INVALID;
+    }
+    DevInfo *dev;
+    rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    DSK_CUDA(launch_lsh_clusters(ix->dev, ix->n_docs, min_count, d_labels, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
 int dsk_jaccard_pairs(const uint32_t *d_sig, int64_t n_rows, int num_perm, const int64_t *d_i, const int64_t *d_j,
                       int64_t m, int32_t *d_count, void *stream) {
     if (n_rows < 0 || num_perm <= 0 || m < 0 || (m > 0 && (!d_sig || !d_i || !d_j || !d_count))) {

@@ -286,3 +286,241 @@ cudaError_t launch_forest_query(const uint32_t *sig, const int32_t *order, int64
 }
 
 }  // namespace dsk
+
+// ---- self-join of the index: candidate pairs and duplicate clusters ----------------------------------------------------
+// Documents i and d (d < i) are a candidate pair iff some band's r-tuples are equal -- d is in MinHashLSH.query(row i),
+// lsh.py:370-432 -- and eq(i, d), the number of the K positions where the rows agree (MinHash.jaccard * K,
+// minhash.py:324), is at least min_count.  Clusters are the connected components of that pair graph, each labelled by its
+// smallest document number.
+namespace dsk {
+
+// Loads and stores of union-find parents that race with hooks: relaxed, so a racing reader sees an old or a new parent.
+// The CPU emulation (-DDSK_EMU) uses the same relaxed atomics of GCC, so ThreadSanitizer checks every other access.
+#ifdef DSK_EMU
+inline int32_t ld_relaxed(const int32_t *p) { return __atomic_load_n(p, __ATOMIC_RELAXED); }
+inline void st_relaxed(int32_t *p, int32_t v) { __atomic_store_n(p, v, __ATOMIC_RELAXED); }
+#else
+__device__ __forceinline__ int32_t ld_relaxed(const int32_t *p) {
+    int32_t v;
+    asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_relaxed(int32_t *p, int32_t v) {
+    asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+#endif
+
+// Lock-free union-find on parent[] with parent[x] <= x at all times.  A hook replaces a root's self-link by a SMALLER
+// root (atomicCAS, so it fails if the root was hooked meanwhile), so every path strictly decreases and the root of each
+// tree is its smallest member.  Path halving may store any ancestor of a non-root x: ancestors never stop being ones.
+__device__ __forceinline__ int32_t uf_find(int32_t *parent, int32_t x) {
+    while (true) {
+        const int32_t p = ld_relaxed(parent + x);
+        if (p == x) return x;
+        const int32_t g = ld_relaxed(parent + p);
+        if (g != p) st_relaxed(parent + x, g);
+        x = g;
+    }
+}
+
+__device__ __forceinline__ void uf_union(int32_t *parent, int32_t a, int32_t b) {
+    while (true) {
+        a = uf_find(parent, a);
+        b = uf_find(parent, b);
+        if (a == b) return;
+        const int32_t hi = a > b ? a : b, lo = a > b ? b : a;
+        if (atomicCAS(parent + hi, hi, lo) == hi) return;
+        a = hi;   // hi was hooked by another thread in between: find both roots again
+        b = lo;
+    }
+}
+
+__global__ void __launch_bounds__(256) uf_init_kernel(int32_t *labels, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        labels[i] = (int32_t)i;
+}
+
+__global__ void __launch_bounds__(256) uf_flatten_kernel(int32_t *labels, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        st_relaxed(labels + i, uf_find(labels, (int32_t)i));
+}
+
+enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2 };
+
+// warp <-> document i, lane <-> band (bands beyond 32 in further rounds), row i staged once in shared memory.  Each lane
+// probes its band's table with the fingerprint of i's own tuple and walks the bucket's chain to its next partner d: d < i,
+// the tuple really equal, and no earlier band with equal tuples (the first matching band emits the pair, as in
+// lsh_query_kernel).  Then the warp counts eq for every lane's pending partner together -- 32 lanes over the two K-word
+// rows and a shuffle reduction, one partner after the other -- and the partners with eq >= min_count are kept:
+//   PAIRS_COUNT  counts[i] = number kept
+//   PAIRS_FILL   written at idx / eq [ptr[i] ...), in no particular order
+//   PAIRS_UNION  united with i in labels[] (nothing materialised)
+template <int MODE>
+__global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t n_docs, int min_count,
+                                                        int64_t *__restrict__ counts, const int64_t *__restrict__ ptr,
+                                                        int32_t *__restrict__ out_idx, int32_t *__restrict__ out_eq,
+                                                        int32_t *labels) {
+    DSK_DYNAMIC_SMEM_T(uint32_t, s_rows, 16);   // [warps][k]
+    const int lane = threadIdx.x & 31;
+    uint32_t *row = s_rows + (int64_t)(threadIdx.x >> 5) * ix.k;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    const uint64_t mask = (uint64_t)ix.cap_slots - 1;
+    const bool need_eq = MODE == PAIRS_FILL || min_count > 0;
+    const unsigned below = (1u << lane) - 1u;
+    for (int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < n_docs; i += warps) {
+        const uint32_t *irow = ix.sig + i * ix.k;
+        __syncwarp();
+        for (int w = lane; w < ix.k; w += 32) row[w] = irow[w];
+        __syncwarp();
+        int64_t total = 0;   // partners kept so far (the same in every lane)
+        for (int band0 = 0; band0 < ix.b; band0 += 32) {
+            const int band = band0 + lane;
+            const uint32_t *it = row + band * ix.r;
+            int32_t d = -1;
+            if (band < ix.b) {
+                const uint64_t fp = band_fp(it, ix.r, band);
+                const uint64_t *tab = ix.slots + (int64_t)band * ix.cap_slots * 2;
+                uint64_t slot = lsh_mix64(fp) & mask;
+                while (true) {
+                    const uint64_t kk = tab[2 * slot];
+                    if (kk == fp) { d = *reinterpret_cast<const int32_t *>(tab + 2 * slot + 1); break; }
+                    if (kk == kEmptyKey) break;
+                    slot = (slot + 1) & mask;
+                }
+            }
+            while (true) {
+                int32_t cand = -1;
+                while (d >= 0) {
+                    const int32_t cur = d;
+                    d = ix.next[(int64_t)cur * ix.b + band];
+                    if (cur < i) {
+                        const uint32_t *drow = ix.sig + (int64_t)cur * ix.k;
+                        if (tuple_eq(drow + band * ix.r, it, ix.r)) {
+                            bool dup = false;
+                            for (int j = 0; j < band && !dup; ++j)
+                                dup = tuple_eq(drow + j * ix.r, row + j * ix.r, ix.r);
+                            if (!dup) { cand = cur; break; }
+                        }
+                    }
+                }
+                const unsigned pending = __ballot_sync(0xFFFFFFFFu, cand >= 0);
+                if (pending == 0u) break;
+                int eq = 0;
+                if (need_eq) {
+                    for (unsigned m = pending; m; m &= m - 1u) {
+                        const int src = __ffs(m) - 1;
+                        const uint32_t *crow = ix.sig + (int64_t)__shfl_sync(0xFFFFFFFFu, cand, src) * ix.k;
+                        int e = 0;
+                        for (int w = lane; w < ix.k; w += 32) e += crow[w] == row[w];
+#pragma unroll
+                        for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xFFFFFFFFu, e, o);
+                        if (lane == src) eq = e;
+                    }
+                }
+                const bool keep = cand >= 0 && eq >= min_count;
+                if (MODE == PAIRS_UNION) {
+                    if (keep) uf_union(labels, (int32_t)i, cand);
+                } else {
+                    const unsigned kept = __ballot_sync(0xFFFFFFFFu, keep);
+                    if (MODE == PAIRS_FILL && keep) {
+                        const int64_t pos = ptr[i] + total + __popc(kept & below);
+                        out_idx[pos] = cand;
+                        out_eq[pos] = eq;
+                    }
+                    total += __popc(kept);
+                }
+            }
+        }
+        if (MODE == PAIRS_COUNT && lane == 0) counts[i] = total;
+    }
+}
+
+// min_count = 0: thread <-> (document i, band).  i is united with the FIRST other member of its band's chain whose tuple
+// equals i's, so the members with one tuple form a star around the first of them in chain order -- the components of the
+// full clique, in time linear in the index (plus the members of other tuples that share the chain's fingerprint).
+__global__ void __launch_bounds__(256) lsh_link_kernel(const LshDev ix, int64_t n_docs, int32_t *labels) {
+    const uint64_t mask = (uint64_t)ix.cap_slots - 1;
+    const int64_t n_pairs = n_docs * ix.b;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n_pairs; p += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t i = p / ix.b;
+        const int band = (int)(p - i * ix.b);
+        const uint32_t *it = ix.sig + i * ix.k + band * ix.r;
+        const uint64_t fp = band_fp(it, ix.r, band);
+        const uint64_t *tab = ix.slots + (int64_t)band * ix.cap_slots * 2;
+        uint64_t slot = lsh_mix64(fp) & mask;
+        int32_t d = -1;
+        while (true) {
+            const uint64_t kk = tab[2 * slot];
+            if (kk == fp) { d = *reinterpret_cast<const int32_t *>(tab + 2 * slot + 1); break; }
+            if (kk == kEmptyKey) break;
+            slot = (slot + 1) & mask;
+        }
+        while (d >= 0) {
+            if (d != i && tuple_eq(ix.sig + (int64_t)d * ix.k + band * ix.r, it, ix.r)) {
+                uf_union(labels, (int32_t)i, d);
+                break;
+            }
+            d = ix.next[(int64_t)d * ix.b + band];
+        }
+    }
+}
+
+// the pair walk's launch shape: up to 8 warps per CTA, each with a K-word row in shared memory
+static cudaError_t pairs_shape(const LshDev &ix, int64_t n_docs, int sm_count, int *warps, unsigned *grid, size_t *smem) {
+    int w = 8;
+    while (w > 1 && (size_t)w * ix.k * 4 > 48 * 1024) w >>= 1;
+    *warps = w;
+    *smem = (size_t)w * ix.k * 4;
+    int64_t g = (n_docs + w - 1) / w;
+    if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
+    *grid = (unsigned)g;
+    cudaError_t e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_COUNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_FILL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_UNION>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+    return e;
+}
+
+// counts != nullptr: counts[i] for every document; else the fill of idx / eq at ptr[i]
+cudaError_t launch_lsh_pairs(const LshDev &ix, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
+                             int32_t *idx, int32_t *eq, int sm_count, cudaStream_t s) {
+    if (n_docs <= 0) return cudaSuccess;
+    int warps;
+    unsigned grid;
+    size_t smem;
+    cudaError_t e = pairs_shape(ix, n_docs, sm_count, &warps, &grid, &smem);
+    if (e != cudaSuccess) return e;
+    if (counts)
+        DSK_LAUNCH(lsh_pairs_kernel<PAIRS_COUNT>, grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr, nullptr,
+                   nullptr, nullptr);
+    else
+        DSK_LAUNCH(lsh_pairs_kernel<PAIRS_FILL>, grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
+                   nullptr);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_lsh_clusters(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels, int sm_count,
+                                cudaStream_t s) {
+    if (n_docs <= 0) return cudaSuccess;
+    int64_t grid = (n_docs + 255) / 256;
+    if (grid > (int64_t)sm_count * 8) grid = (int64_t)sm_count * 8;
+    DSK_LAUNCH(uf_init_kernel, (unsigned)grid, 256, 0, s, labels, n_docs);
+    if (min_count == 0) {
+        int64_t lg = (n_docs * ix.b + 255) / 256;
+        if (lg > (int64_t)sm_count * 8) lg = (int64_t)sm_count * 8;
+        DSK_LAUNCH(lsh_link_kernel, (unsigned)lg, 256, 0, s, ix, n_docs, labels);
+    } else {
+        int warps;
+        unsigned pg;
+        size_t smem;
+        cudaError_t e = pairs_shape(ix, n_docs, sm_count, &warps, &pg, &smem);
+        if (e != cudaSuccess) return e;
+        DSK_LAUNCH(lsh_pairs_kernel<PAIRS_UNION>, pg, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr, nullptr,
+                   nullptr, labels);
+    }
+    DSK_LAUNCH(uf_flatten_kernel, (unsigned)grid, 256, 0, s, labels, n_docs);
+    return cudaGetLastError();
+}
+
+}  // namespace dsk

@@ -615,3 +615,61 @@ class GpuLSH:
             ids = idx[ptr[q]:ptr[q + 1]]
             out.append([self.keys[i] for i in ids] if self.keys else ids.tolist())
         return out
+
+    # -- self-join: near-duplicate pairs and clusters of the indexed documents ------------------------------------------
+    def candidate_pairs(self, min_jaccard: Optional[float] = None, to_host: bool = True):
+        """Every candidate pair among the ``n = len(self)`` indexed documents, once, as CSR arrays
+        ``(ptr int64[n+1], idx int32[M], eq int32[M])``.
+
+        ``idx[ptr[i]:ptr[i+1]]`` holds (unordered) the documents ``d < i`` that ``query`` returns for document i's own row,
+        and ``eq`` the number of the ``num_perm`` positions where the two rows agree, so ``eq / num_perm`` is
+        ``MinHash.jaccard`` of the pair.  ``min_jaccard`` keeps only the pairs with ``MinHash.jaccard >= min_jaccard``.
+        Runs on the device: one warp per document walks the document's buckets and compares the rows the index holds."""
+        import torch
+        mc = _jaccard_min_count(min_jaccard, self.h)
+        n = len(self)
+        lib = nv.load()
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream().cuda_stream
+            counts = torch.empty((max(n, 1),), dtype=torch.int64, device=dev)
+            ptr = torch.empty((n + 1,), dtype=torch.int64, device=dev)
+            scratch = torch.empty((n // 1024 + 2,), dtype=torch.int64, device=dev)
+            nv.check(lib.dsk_lsh_pairs_count(self._h, mc, counts.data_ptr(), st))
+            nv.check(lib.dsk_exclusive_scan(counts.data_ptr(), n, ptr.data_ptr(), scratch.data_ptr(), st))
+            total = int(ptr[n].item())
+            idx = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
+            eq = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
+            nv.check(lib.dsk_lsh_pairs_fill(self._h, mc, ptr.data_ptr(), idx.data_ptr(), eq.data_ptr(), st))
+            idx, eq = idx[:total], eq[:total]
+        if to_host:
+            return ptr.cpu().numpy(), idx.cpu().numpy(), eq.cpu().numpy()
+        return ptr, idx, eq
+
+    def duplicate_clusters(self, min_jaccard: Optional[float] = None, to_host: bool = True):
+        """``labels int32[n]``: ``labels[i]`` is the smallest document number of i's connected component in the graph of
+        ``candidate_pairs(min_jaccard)``.  Deterministic; ``labels[i] == i`` marks the one document of each cluster a
+        de-duplication keeps, and ``keys`` (when set) maps labels to user keys.
+
+        Without ``min_jaccard`` each document is linked to the first equal member of each of its buckets, which takes
+        time linear in the index however large its buckets are.  With ``min_jaccard`` every candidate pair is verified,
+        which takes time quadratic in the size of each bucket."""
+        import torch
+        mc = _jaccard_min_count(min_jaccard, self.h)
+        n = len(self)
+        with torch.cuda.device(self.device):
+            labels = torch.empty((max(n, 1),), dtype=torch.int32, device=torch.device("cuda", self.device))
+            nv.check(nv.load().dsk_lsh_clusters(self._h, mc, labels.data_ptr(), torch.cuda.current_stream().cuda_stream))
+            labels = labels[:n]
+        return labels.cpu().numpy() if to_host else labels
+
+
+def _jaccard_min_count(min_jaccard: Optional[float], num_perm: int) -> int:
+    """The smallest count c in 0..num_perm with ``float(c) / float(num_perm) >= min_jaccard`` -- exactly the pairs
+    ``MinHash.jaccard(...) >= min_jaccard`` keeps (minhash.py:324 divides in float64 the same way).  None -> 0."""
+    if min_jaccard is None:
+        return 0
+    t = float(min_jaccard)
+    if not 0.0 <= t <= 1.0:
+        raise ValueError("min_jaccard must be in [0.0, 1.0]")
+    return next(c for c in range(num_perm + 1) if float(c) / float(num_perm) >= t)   # c = num_perm always qualifies

@@ -222,7 +222,17 @@ DSK_API int dsk_wmh_minhash(const dsk_wmh *g, const float *d_v, int64_t n, int64
  *   dsk_exclusive_scan   d_out[0..n] = exclusive prefix sums of d_in[0..n-1] (d_out[n] = total);
  *                        d_scratch holds at least n/1024 + 2 int64
  *   dsk_lsh_query_fill   writes each query's candidates (document numbers, unordered like the
- *                        reference's list(set), lsh.py:432) at d_idx[d_ptr[q] .. d_ptr[q+1]) */
+ *                        reference's list(set), lsh.py:432) at d_idx[d_ptr[q] .. d_ptr[q+1])
+ * Self-join of the n_docs documents inserted so far.  i and d < i are a candidate pair iff d is a candidate of
+ * query(row i), and eq(i, d) = number of the num_perm positions where the two rows agree (MinHash.jaccard * num_perm,
+ * minhash.py:324).  min_count in [0, num_perm] keeps the pairs with eq >= min_count (0 keeps all).
+ *   dsk_lsh_pairs_count  d_counts[i] = number of kept partners d < i of document i
+ *   dsk_lsh_pairs_fill   after dsk_exclusive_scan of the counts: writes i's partners at d_idx[d_ptr[i] .. d_ptr[i+1])
+ *                        (unordered) and their eq at the same positions of d_eq
+ *   dsk_lsh_clusters     d_labels[i] = smallest document number of i's connected component of the kept pairs' graph
+ *                        (deterministic; d_labels is the union-find's parent array, no other workspace).  min_count = 0
+ *                        links each document to the first equal member of each of its buckets: linear in the index.
+ *                        min_count > 0 walks every pair: quadratic in the size of each bucket. */
 typedef struct dsk_lsh dsk_lsh;
 DSK_API int dsk_lsh_create(int num_perm, int b, int r, int64_t capacity_docs, int device, dsk_lsh **out);
 DSK_API void dsk_lsh_destroy(dsk_lsh *ix);
@@ -234,6 +244,10 @@ DSK_API int dsk_lsh_query_count(const dsk_lsh *ix, const uint32_t *d_qsig, int64
 DSK_API int dsk_lsh_query_fill(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, const int64_t *d_ptr,
                                int32_t *d_idx, void *stream);
 DSK_API int dsk_exclusive_scan(const int64_t *d_in, int64_t n, int64_t *d_out, int64_t *d_scratch, void *stream);
+DSK_API int dsk_lsh_pairs_count(const dsk_lsh *ix, int min_count, int64_t *d_counts, void *stream);
+DSK_API int dsk_lsh_pairs_fill(const dsk_lsh *ix, int min_count, const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq,
+                               void *stream);
+DSK_API int dsk_lsh_clusters(const dsk_lsh *ix, int min_count, int32_t *d_labels, void *stream);
 
 /* ---- Jaccard estimate -----------------------------------------------------------------------
  * d_count[p] = number of positions where rows d_i[p] and d_j[p] of the [n_rows, num_perm] u32

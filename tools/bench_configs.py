@@ -32,8 +32,9 @@ def ev_time(fn, iters=3, warm=1):
     return e0.elapsed_time(e1) / iters
 
 
-def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False):
-    """10M x 128 tokens, K=256 + LSH(0.8) insert + query (here n_docs on one GPU)."""
+def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False):
+    """10M x 128 tokens, K=256 + LSH(0.8) insert + query (here n_docs on one GPU).  dedup_leg: also the self-join of
+    the index (candidate_pairs, duplicate_clusters with and without min_jaccard=0.8) against the host flow it replaces."""
     perms = _make_permutations(k, 1)
     g = torch.Generator(device="cuda").manual_seed(3)
     tok = torch.randint(-2 ** 31, 2 ** 31 - 1, (n_docs, t), dtype=torch.int32, device="cuda", generator=g)
@@ -98,6 +99,7 @@ def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False):
     for row in hs[:5000]:
         ref.query(row)
     cpu_q = (time.perf_counter() - t0) / 5000
+    dedup = c3_dedup(lsh, src, dst, ref, hs) if dedup_leg else {}
     return {"config": "C3 (1 GPU)", "docs": n_docs, "tokens": t, "num_perm": k, "b": lsh.b, "r": lsh.r,
             "signature_ms": ms_sig, "signatures_per_s": n_docs / ms_sig * 1e3,
             "lsh_insert_ms": ms_ins, "lsh_insert_docs_per_s": n_docs / ms_ins * 1e3,
@@ -105,7 +107,42 @@ def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False):
             "two_step_signatures_plus_insert_ms": ms_sig + ms_ins, "fused_candidates_identical": same,
             "lsh_query_ms": ms_q, "queries": n_query, "lsh_queries_per_s": n_query / ms_q * 1e3,
             "candidates_total": int(ptr[-1].item()),
-            "cpu_oracle_insert_us_per_doc": cpu_ins * 1e6, "cpu_oracle_query_us_per_doc": cpu_q * 1e6}
+            "cpu_oracle_insert_us_per_doc": cpu_ins * 1e6, "cpu_oracle_query_us_per_doc": cpu_q * 1e6, **dedup}
+
+
+def c3_dedup(lsh, src, dst, ref, hs, min_jaccard=0.8):
+    """Self-join of the C3 index on the device, warmed up, timed with CUDA events; beside it, on the first len(hs)
+    documents (already in the dict oracle ``ref``), the host flow it replaces: DictLSH.query per document, oracle_np.jaccard
+    per pair, scipy connected components of the pairs with jaccard >= min_jaccard."""
+    from scipy.sparse import coo_matrix
+    from scipy.sparse.csgraph import connected_components
+    n = len(lsh)
+    ms_pairs = ev_time(lambda: lsh.candidate_pairs(to_host=False))
+    ms_cl = ev_time(lambda: lsh.duplicate_clusters(to_host=False))
+    ms_cl_t = ev_time(lambda: lsh.duplicate_clusters(min_jaccard, to_host=False))
+    ptr, _, _ = lsh.candidate_pairs(to_host=False)
+    pairs = int(ptr[-1].item())
+    out = {"dedup_pairs": pairs, "dedup_candidate_pairs_ms": ms_pairs, "dedup_pairs_per_s": pairs / ms_pairs * 1e3,
+           "dedup_candidate_pairs_docs_per_s": n / ms_pairs * 1e3,
+           "dedup_clusters_ms": ms_cl, "dedup_clusters_docs_per_s": n / ms_cl * 1e3,
+           "dedup_min_jaccard": min_jaccard, "dedup_clusters_min_jaccard_ms": ms_cl_t,
+           "dedup_clusters_min_jaccard_docs_per_s": n / ms_cl_t * 1e3}
+    ar = torch.arange(n, dtype=torch.int32, device="cuda")
+    for tag, t in (("", None), ("_min_jaccard", min_jaccard)):
+        labels = lsh.duplicate_clusters(t, to_host=False)
+        out["dedup_clusters" + tag] = int((labels == ar).sum().item())
+        out["dedup_planted_together" + tag] = float((labels[src] == labels[dst]).float().mean().item())
+    t0 = time.perf_counter()
+    ii, dd = [], []
+    for i, row in enumerate(hs):
+        for d in ref.query(row):
+            if d < i and o.jaccard(row, hs[d]) >= min_jaccard:
+                ii.append(i)
+                dd.append(d)
+    ns = len(hs)
+    connected_components(coo_matrix((np.ones(len(ii)), (ii, dd)), shape=(ns, ns)), directed=False)
+    out["dedup_host_flow_us_per_doc"] = (time.perf_counter() - t0) / ns * 1e6
+    return out
 
 
 def c4(n_vec, dim=4096, ss=128):
@@ -177,9 +214,11 @@ if __name__ == "__main__":
     ap.add_argument("--c5-rows", type=int, default=100_000)
     ap.add_argument("--c3-fused", action="store_true",
                     help="also time GpuLSH.insert_tokens (fused signatures + insert); tools/diag_fused.py times it alone")
+    ap.add_argument("--c3-dedup", action="store_true",
+                    help="also time GpuLSH.candidate_pairs / duplicate_clusters on the C3 index and the host flow they replace")
     a = ap.parse_args()
     if a.c3_docs > 0:
-        print(json.dumps(c3(a.c3_docs, fused_leg=a.c3_fused)), flush=True)
+        print(json.dumps(c3(a.c3_docs, fused_leg=a.c3_fused, dedup_leg=a.c3_dedup)), flush=True)
     for fn, arg in ((c4, a.c4_vecs), (c5, a.c5_rows)):
         if arg > 0:
             print(json.dumps(fn(arg)), flush=True)
