@@ -159,6 +159,9 @@ struct dsk_lsh {
     int device = 0;
     LshDev dev{};
     int64_t n_docs = 0;
+    uint32_t *removed = nullptr;   // removal bitmap, (cap_docs + 31) / 32 words: allocated by the first dsk_lsh_remove
+    bool has_removals = false;     // a dsk_lsh_remove since the last compaction: the walks run their removal-aware kernels
+    const uint32_t *walk_bitmap() const { return has_removals ? removed : nullptr; }
 };
 
 extern "C" {
@@ -689,6 +692,7 @@ void dsk_lsh_destroy(dsk_lsh *ix) {
     if (ix->dev.sig) cudaFree(ix->dev.sig);
     if (ix->dev.slots) cudaFree(ix->dev.slots);
     if (ix->dev.next) cudaFree(ix->dev.next);
+    if (ix->removed) cudaFree(ix->removed);
     cudaSetDevice(prev);
     delete ix;
 }
@@ -792,7 +796,7 @@ int dsk_lsh_query_count(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, i
     int rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(launch_lsh_query(ix->dev, d_qsig, nq, ix->n_docs, d_counts, nullptr, nullptr, 0, dev->sm_count,
+    DSK_CUDA(launch_lsh_query(ix->dev, d_qsig, nq, ix->n_docs, d_counts, nullptr, nullptr, 0, ix->walk_bitmap(), dev->sm_count,
                               (cudaStream_t)stream));
     return DSK_OK;
 }
@@ -807,7 +811,7 @@ int dsk_lsh_query_fill(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, co
     int rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(launch_lsh_query(ix->dev, d_qsig, nq, ix->n_docs, nullptr, d_ptr, d_idx, 1, dev->sm_count,
+    DSK_CUDA(launch_lsh_query(ix->dev, d_qsig, nq, ix->n_docs, nullptr, d_ptr, d_idx, 1, ix->walk_bitmap(), dev->sm_count,
                               (cudaStream_t)stream));
     return DSK_OK;
 }
@@ -844,7 +848,7 @@ int dsk_lsh_pairs_count(const dsk_lsh *ix, int min_count, int64_t *d_counts, voi
     rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->n_docs, min_count, d_counts, nullptr, nullptr, nullptr, dev->sm_count,
+    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->n_docs, min_count, d_counts, nullptr, nullptr, nullptr, ix->walk_bitmap(), dev->sm_count,
                               (cudaStream_t)stream));
     return DSK_OK;
 }
@@ -861,7 +865,7 @@ int dsk_lsh_pairs_fill(const dsk_lsh *ix, int min_count, const int64_t *d_ptr, i
     rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->n_docs, min_count, nullptr, d_ptr, d_idx, d_eq, dev->sm_count,
+    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->n_docs, min_count, nullptr, d_ptr, d_idx, d_eq, ix->walk_bitmap(), dev->sm_count,
                               (cudaStream_t)stream));
     return DSK_OK;
 }
@@ -877,7 +881,99 @@ int dsk_lsh_clusters(const dsk_lsh *ix, int min_count, int32_t *d_labels, void *
     rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(launch_lsh_clusters(ix->dev, ix->n_docs, min_count, d_labels, dev->sm_count, (cudaStream_t)stream));
+    DSK_CUDA(launch_lsh_clusters(ix->dev, ix->n_docs, min_count, d_labels, ix->walk_bitmap(), dev->sm_count,
+                                 (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+static int check_ids(const char *who, const dsk_lsh *ix, const void *d_docs, int64_t n, const void *d_out) {
+    if (!ix) {
+        set_error("%s: null handle", who);
+        return DSK_ERR_INVALID;
+    }
+    if (n < 0) {
+        set_error("%s: n must be >= 0 (got %lld)", who, (long long)n);
+        return DSK_ERR_INVALID;
+    }
+    if (n > 0 && (!d_docs || !d_out)) {
+        set_error("%s: null buffer", who);
+        return DSK_ERR_INVALID;
+    }
+    return DSK_OK;
+}
+
+int dsk_lsh_remove(dsk_lsh *ix, const int32_t *d_docs, int64_t n, int64_t *d_status, void *stream) {
+    int rc = check_ids("dsk_lsh_remove", ix, d_docs, n, d_status);
+    if (rc || n == 0) return rc;
+    DevInfo *dev;
+    rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    const size_t words = (size_t)(ix->dev.cap_docs + 31) / 32;
+    if (!ix->removed) {   // an index that never removes anything keeps the memory dsk_lsh_create gave it
+        uint32_t *bits = nullptr;
+        DSK_CUDA(cudaMalloc(&bits, words * sizeof(uint32_t)));
+        const cudaError_t e = cudaMemsetAsync(bits, 0, words * sizeof(uint32_t), (cudaStream_t)stream);
+        if (e != cudaSuccess) {
+            cudaFree(bits);
+            return cuda_fail(e, "dsk_lsh_remove bitmap");
+        }
+        ix->removed = bits;
+    }
+    ix->has_removals = true;
+    DSK_CUDA(launch_lsh_remove(ix->removed, d_docs, n, ix->n_docs, d_status, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_lsh_alive(const dsk_lsh *ix, const int32_t *d_docs, int64_t n, uint8_t *d_out, void *stream) {
+    int rc = check_ids("dsk_lsh_alive", ix, d_docs, n, d_out);
+    if (rc || n == 0) return rc;
+    DevInfo *dev;
+    rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    DSK_CUDA(launch_lsh_alive(ix->walk_bitmap(), d_docs, n, ix->n_docs, d_out, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+size_t dsk_lsh_compact_workspace_size(const dsk_lsh *ix) {
+    return ix ? lsh_compact_workspace_bytes(ix->n_docs, ix->dev.k) : 0;
+}
+
+int dsk_lsh_compact(dsk_lsh *ix, int32_t *d_remap, void *d_ws, size_t ws_bytes, void *stream) {
+    if (!ix) {
+        set_error("dsk_lsh_compact: null handle");
+        return DSK_ERR_INVALID;
+    }
+    const int64_t n = ix->n_docs;
+    const size_t need = lsh_compact_workspace_bytes(n, ix->dev.k);
+    if (n > 0 && (!d_remap || !d_ws)) {
+        set_error("dsk_lsh_compact: null buffer");
+        return DSK_ERR_INVALID;
+    }
+    if (n > 0 && (((uintptr_t)d_ws & 15) != 0 || ws_bytes < need)) {
+        set_error("dsk_lsh_compact: the workspace must be 16-byte aligned and hold dsk_lsh_compact_workspace_size() = %zu bytes (got %zu)",
+                  need, ws_bytes);
+        return DSK_ERR_INVALID;
+    }
+    if (n == 0) {
+        ix->has_removals = false;
+        return DSK_OK;
+    }
+    DevInfo *dev;
+    int rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (!ix->has_removals) {   // nothing removed: the identity remap, no synchronisation, no rebuild
+        DSK_CUDA(launch_lsh_identity(d_remap, n, dev->sm_count, s));
+        return DSK_OK;
+    }
+    int64_t m = n;
+    DSK_CUDA(lsh_compact(ix->dev, ix->removed, n, d_remap, d_ws, &m, dev->sm_count, s));
+    DSK_CUDA(cudaMemsetAsync(ix->removed, 0, (size_t)(n + 31) / 32 * sizeof(uint32_t), s));
+    ix->has_removals = false;
+    ix->n_docs = m;
     return DSK_OK;
 }
 

@@ -121,15 +121,29 @@ struct LshDev {
 };
 cudaError_t launch_lsh_insert(const LshDev &ix, const uint32_t *new_sig, int64_t doc0, int64_t n_new, int sm_count,
                               cudaStream_t s);
+// `removed`: the removal bitmap when the index has removals since its last compaction (the removal-aware kernels run), else
+// nullptr (the kernels that run when nothing was ever removed)
 cudaError_t launch_lsh_query(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int64_t *counts,
-                             const int64_t *ptr, int32_t *out, int fill, int sm_count, cudaStream_t s);
+                             const int64_t *ptr, int32_t *out, int fill, const uint32_t *removed, int sm_count,
+                             cudaStream_t s);
+cudaError_t launch_lsh_query(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int64_t *counts,
+                             const int64_t *ptr, int32_t *out, int fill, int sm_count, cudaStream_t s);   // nothing removed
 cudaError_t launch_exclusive_scan(const int64_t *in, int64_t n, int64_t *out, int64_t *scratch, cudaStream_t s);
 // self-join of the first n_docs documents (d < i, a band's tuple equal, eq >= min_count): per-document counts, or the fill
 // of idx / eq at ptr[i] (counts == nullptr); clusters: labels[i] = smallest document of i's component of the pair graph
 cudaError_t launch_lsh_pairs(const LshDev &ix, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
-                             int32_t *idx, int32_t *eq, int sm_count, cudaStream_t s);
-cudaError_t launch_lsh_clusters(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels, int sm_count,
-                                cudaStream_t s);
+                             int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s);
+cudaError_t launch_lsh_clusters(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels, const uint32_t *removed,
+                                int sm_count, cudaStream_t s);
+// removal (bits of the bitmap) and compaction of the index
+cudaError_t launch_lsh_remove(uint32_t *removed, const int32_t *docs, int64_t n, int64_t n_docs, int64_t *status,
+                              int sm_count, cudaStream_t s);
+cudaError_t launch_lsh_alive(const uint32_t *removed, const int32_t *docs, int64_t n, int64_t n_docs, uint8_t *out,
+                             int sm_count, cudaStream_t s);
+size_t lsh_compact_workspace_bytes(int64_t n_docs, int k);
+cudaError_t launch_lsh_identity(int32_t *remap, int64_t n, int sm_count, cudaStream_t s);   // remap[i] = i
+cudaError_t lsh_compact(const LshDev &ix, const uint32_t *removed, int64_t n_docs, int32_t *remap, void *ws, int64_t *m,
+                        int sm_count, cudaStream_t s);
 
 cudaError_t launch_jaccard_pairs(const uint32_t *sig, int64_t n_rows, int k, const int64_t *ia, const int64_t *ib,
                                  int64_t m, int32_t *out, int sm_count, cudaStream_t s);

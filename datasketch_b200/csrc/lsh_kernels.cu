@@ -23,6 +23,14 @@ __device__ __forceinline__ bool tuple_eq(const uint32_t *a, const uint32_t *b, i
     return eq;
 }
 
+// Removal bitmap (dsk_lsh_remove): bit d of removed[d / 32] set = document d was removed since the last compaction.  The
+// walks below take it through a template flag RM; the RM = false instantiations never read it and are the kernels that
+// ran before removal existed.  Removed documents stay in the bucket chains until dsk_lsh_compact, because they link the
+// members behind them: a walk passes through them and never counts, emits, verifies or unites one.
+__device__ __forceinline__ bool is_removed(const uint32_t *removed, int64_t d) {
+    return (__ldg(removed + (d >> 5)) >> (d & 31)) & 1u;
+}
+
 // CTA <-> tile of D = 256 / b new documents.  The tile's rows are contiguous: they are read ONCE with fully coalesced
 // loads, each value going to the index's own copy of the signatures (candidates are verified on the r-tuples
 // themselves) and to shared memory; then thread <-> (document, band) takes its r-tuple from shared memory for the
@@ -66,10 +74,12 @@ __global__ void __launch_bounds__(256) lsh_insert_kernel(const LshDev ix, const 
 
 // warp <-> query, lane <-> band (bands beyond 32 are handled in further rounds).
 // FILL = false: counts[q] = number of distinct candidates.  FILL = true: writes them at out[ptr[q]...].
-template <bool FILL>
+// RM: removed documents are no candidates.
+template <bool FILL, bool RM>
 __global__ void __launch_bounds__(256) lsh_query_kernel(const LshDev ix, const uint32_t *__restrict__ qsig, int64_t nq,
                                                         int64_t n_docs, int64_t *__restrict__ counts,
-                                                        const int64_t *__restrict__ ptr, int32_t *__restrict__ out) {
+                                                        const int64_t *__restrict__ ptr, int32_t *__restrict__ out,
+                                                        const uint32_t *__restrict__ removed) {
     const int lane = threadIdx.x & 31;
     const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
     const uint64_t mask = (uint64_t)ix.cap_slots - 1;
@@ -97,7 +107,7 @@ __global__ void __launch_bounds__(256) lsh_query_kernel(const LshDev ix, const u
                         slot = (slot + 1) & mask;
                     }
                     while (d >= 0) {
-                        if (d < n_docs) {
+                        if (d < n_docs && !(RM && is_removed(removed, d))) {
                             const uint32_t *drow = ix.sig + (int64_t)d * ix.k;
                             if (tuple_eq(drow + (int64_t)band * ix.r, qt, ix.r)) {
                                 bool dup = false;  // already produced by an earlier band?
@@ -181,13 +191,24 @@ cudaError_t launch_lsh_insert(const LshDev &ix, const uint32_t *new_sig, int64_t
 }
 
 cudaError_t launch_lsh_query(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int64_t *counts,
-                             const int64_t *ptr, int32_t *out, int fill, int sm_count, cudaStream_t s) {
+                             const int64_t *ptr, int32_t *out, int fill, const uint32_t *removed, int sm_count,
+                             cudaStream_t s) {
     if (nq <= 0) return cudaSuccess;
     int64_t grid = (nq + 7) / 8;
     if (grid > (int64_t)sm_count * 8) grid = (int64_t)sm_count * 8;
-    if (fill) DSK_LAUNCH((lsh_query_kernel<true>), (unsigned)grid, 256, 0, s, ix, qsig, nq, n_docs, counts, ptr, out);
-    else DSK_LAUNCH((lsh_query_kernel<false>), (unsigned)grid, 256, 0, s, ix, qsig, nq, n_docs, counts, ptr, out);
+    if (removed) {
+        if (fill) DSK_LAUNCH((lsh_query_kernel<true, true>), (unsigned)grid, 256, 0, s, ix, qsig, nq, n_docs, counts, ptr, out, removed);
+        else DSK_LAUNCH((lsh_query_kernel<false, true>), (unsigned)grid, 256, 0, s, ix, qsig, nq, n_docs, counts, ptr, out, removed);
+    } else {
+        if (fill) DSK_LAUNCH((lsh_query_kernel<true, false>), (unsigned)grid, 256, 0, s, ix, qsig, nq, n_docs, counts, ptr, out, nullptr);
+        else DSK_LAUNCH((lsh_query_kernel<false, false>), (unsigned)grid, 256, 0, s, ix, qsig, nq, n_docs, counts, ptr, out, nullptr);
+    }
     return cudaGetLastError();
+}
+
+cudaError_t launch_lsh_query(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int64_t *counts,
+                             const int64_t *ptr, int32_t *out, int fill, int sm_count, cudaStream_t s) {
+    return launch_lsh_query(ix, qsig, nq, n_docs, counts, ptr, out, fill, nullptr, sm_count, s);
 }
 
 // out has n + 1 entries; scratch needs (n / 1024 + 2) int64
@@ -340,9 +361,14 @@ __global__ void __launch_bounds__(256) uf_init_kernel(int32_t *labels, int64_t n
         labels[i] = (int32_t)i;
 }
 
-__global__ void __launch_bounds__(256) uf_flatten_kernel(int32_t *labels, int64_t n) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        st_relaxed(labels + i, uf_find(labels, (int32_t)i));
+// RM: a removed document gets the label -1.  Nothing ever hooks a removed document (the walks never unite one), so it is
+// a root of its own that no other document's path passes through, and its plain store races with no find.
+template <bool RM>
+__global__ void __launch_bounds__(256) uf_flatten_kernel(int32_t *labels, int64_t n, const uint32_t *__restrict__ removed) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        if (RM && is_removed(removed, i)) labels[i] = -1;
+        else st_relaxed(labels + i, uf_find(labels, (int32_t)i));
+    }
 }
 
 enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2 };
@@ -355,11 +381,13 @@ enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2 };
 //   PAIRS_COUNT  counts[i] = number kept
 //   PAIRS_FILL   written at idx / eq [ptr[i] ...), in no particular order
 //   PAIRS_UNION  united with i in labels[] (nothing materialised)
-template <int MODE>
+// RM: a removed i has no partners (its whole iteration is skipped, warp-uniformly; PAIRS_COUNT still writes counts[i] = 0),
+// and a removed d is no partner.
+template <int MODE, bool RM>
 __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t n_docs, int min_count,
                                                         int64_t *__restrict__ counts, const int64_t *__restrict__ ptr,
                                                         int32_t *__restrict__ out_idx, int32_t *__restrict__ out_eq,
-                                                        int32_t *labels) {
+                                                        int32_t *labels, const uint32_t *__restrict__ removed) {
     DSK_DYNAMIC_SMEM_T(uint32_t, s_rows, 16);   // [warps][k]
     const int lane = threadIdx.x & 31;
     uint32_t *row = s_rows + (int64_t)(threadIdx.x >> 5) * ix.k;
@@ -368,6 +396,10 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
     const bool need_eq = MODE == PAIRS_FILL || min_count > 0;
     const unsigned below = (1u << lane) - 1u;
     for (int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < n_docs; i += warps) {
+        if (RM && is_removed(removed, i)) {
+            if (MODE == PAIRS_COUNT && lane == 0) counts[i] = 0;
+            continue;
+        }
         const uint32_t *irow = ix.sig + i * ix.k;
         __syncwarp();
         for (int w = lane; w < ix.k; w += 32) row[w] = irow[w];
@@ -393,7 +425,7 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
                 while (d >= 0) {
                     const int32_t cur = d;
                     d = ix.next[(int64_t)cur * ix.b + band];
-                    if (cur < i) {
+                    if (cur < i && !(RM && is_removed(removed, cur))) {
                         const uint32_t *drow = ix.sig + (int64_t)cur * ix.k;
                         if (tuple_eq(drow + band * ix.r, it, ix.r)) {
                             bool dup = false;
@@ -438,11 +470,18 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
 // min_count = 0: thread <-> (document i, band).  i is united with the FIRST other member of its band's chain whose tuple
 // equals i's, so the members with one tuple form a star around the first of them in chain order -- the components of the
 // full clique, in time linear in the index (plus the members of other tuples that share the chain's fingerprint).
-__global__ void __launch_bounds__(256) lsh_link_kernel(const LshDev ix, int64_t n_docs, int32_t *labels) {
+// RM: a removed i does nothing, and a remaining i is united with the first OTHER REMAINING member with its tuple.  The
+// star argument holds for the remaining members alone: let f be the first remaining member with the tuple in chain order;
+// every other remaining member with the tuple meets f first and unites with it, and f unites with the second one.  So
+// the remaining members with one tuple are connected, and no removed document is ever united.
+template <bool RM>
+__global__ void __launch_bounds__(256) lsh_link_kernel(const LshDev ix, int64_t n_docs, int32_t *labels,
+                                                       const uint32_t *__restrict__ removed) {
     const uint64_t mask = (uint64_t)ix.cap_slots - 1;
     const int64_t n_pairs = n_docs * ix.b;
     for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n_pairs; p += (int64_t)gridDim.x * blockDim.x) {
         const int64_t i = p / ix.b;
+        if (RM && is_removed(removed, i)) continue;
         const int band = (int)(p - i * ix.b);
         const uint32_t *it = ix.sig + i * ix.k + band * ix.r;
         const uint64_t fp = band_fp(it, ix.r, band);
@@ -456,7 +495,7 @@ __global__ void __launch_bounds__(256) lsh_link_kernel(const LshDev ix, int64_t 
             slot = (slot + 1) & mask;
         }
         while (d >= 0) {
-            if (d != i && tuple_eq(ix.sig + (int64_t)d * ix.k + band * ix.r, it, ix.r)) {
+            if (d != i && !(RM && is_removed(removed, d)) && tuple_eq(ix.sig + (int64_t)d * ix.k + band * ix.r, it, ix.r)) {
                 uf_union(labels, (int32_t)i, d);
                 break;
             }
@@ -466,6 +505,7 @@ __global__ void __launch_bounds__(256) lsh_link_kernel(const LshDev ix, int64_t 
 }
 
 // the pair walk's launch shape: up to 8 warps per CTA, each with a K-word row in shared memory
+template <bool RM>
 static cudaError_t pairs_shape(const LshDev &ix, int64_t n_docs, int sm_count, int *warps, unsigned *grid, size_t *smem) {
     int w = 8;
     while (w > 1 && (size_t)w * ix.k * 4 > 48 * 1024) w >>= 1;
@@ -474,53 +514,249 @@ static cudaError_t pairs_shape(const LshDev &ix, int64_t n_docs, int sm_count, i
     int64_t g = (n_docs + w - 1) / w;
     if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
     *grid = (unsigned)g;
-    cudaError_t e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_COUNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+    cudaError_t e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_COUNT, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_FILL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+        e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_FILL, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_UNION>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+        e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_UNION, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
     return e;
 }
 
-// counts != nullptr: counts[i] for every document; else the fill of idx / eq at ptr[i]
-cudaError_t launch_lsh_pairs(const LshDev &ix, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
-                             int32_t *idx, int32_t *eq, int sm_count, cudaStream_t s) {
-    if (n_docs <= 0) return cudaSuccess;
+template <bool RM>
+static cudaError_t launch_pairs_t(const LshDev &ix, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
+                                  int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s) {
     int warps;
     unsigned grid;
     size_t smem;
-    cudaError_t e = pairs_shape(ix, n_docs, sm_count, &warps, &grid, &smem);
+    cudaError_t e = pairs_shape<RM>(ix, n_docs, sm_count, &warps, &grid, &smem);
     if (e != cudaSuccess) return e;
     if (counts)
-        DSK_LAUNCH(lsh_pairs_kernel<PAIRS_COUNT>, grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr, nullptr,
-                   nullptr, nullptr);
+        DSK_LAUNCH((lsh_pairs_kernel<PAIRS_COUNT, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr,
+                   nullptr, nullptr, nullptr, removed);
     else
-        DSK_LAUNCH(lsh_pairs_kernel<PAIRS_FILL>, grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
-                   nullptr);
+        DSK_LAUNCH((lsh_pairs_kernel<PAIRS_FILL, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
+                   nullptr, removed);
     return cudaGetLastError();
 }
 
-cudaError_t launch_lsh_clusters(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels, int sm_count,
-                                cudaStream_t s) {
+// counts != nullptr: counts[i] for every document; else the fill of idx / eq at ptr[i].  removed != nullptr: the
+// removal-aware walk.
+cudaError_t launch_lsh_pairs(const LshDev &ix, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
+                             int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s) {
     if (n_docs <= 0) return cudaSuccess;
+    if (removed) return launch_pairs_t<true>(ix, n_docs, min_count, counts, ptr, idx, eq, removed, sm_count, s);
+    return launch_pairs_t<false>(ix, n_docs, min_count, counts, ptr, idx, eq, nullptr, sm_count, s);
+}
+
+template <bool RM>
+static cudaError_t launch_clusters_t(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels,
+                                     const uint32_t *removed, int sm_count, cudaStream_t s) {
     int64_t grid = (n_docs + 255) / 256;
     if (grid > (int64_t)sm_count * 8) grid = (int64_t)sm_count * 8;
     DSK_LAUNCH(uf_init_kernel, (unsigned)grid, 256, 0, s, labels, n_docs);
     if (min_count == 0) {
         int64_t lg = (n_docs * ix.b + 255) / 256;
         if (lg > (int64_t)sm_count * 8) lg = (int64_t)sm_count * 8;
-        DSK_LAUNCH(lsh_link_kernel, (unsigned)lg, 256, 0, s, ix, n_docs, labels);
+        DSK_LAUNCH(lsh_link_kernel<RM>, (unsigned)lg, 256, 0, s, ix, n_docs, labels, removed);
     } else {
         int warps;
         unsigned pg;
         size_t smem;
-        cudaError_t e = pairs_shape(ix, n_docs, sm_count, &warps, &pg, &smem);
+        cudaError_t e = pairs_shape<RM>(ix, n_docs, sm_count, &warps, &pg, &smem);
         if (e != cudaSuccess) return e;
-        DSK_LAUNCH(lsh_pairs_kernel<PAIRS_UNION>, pg, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr, nullptr,
-                   nullptr, labels);
+        DSK_LAUNCH((lsh_pairs_kernel<PAIRS_UNION, RM>), pg, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr,
+                   nullptr, nullptr, labels, removed);
     }
-    DSK_LAUNCH(uf_flatten_kernel, (unsigned)grid, 256, 0, s, labels, n_docs);
+    DSK_LAUNCH(uf_flatten_kernel<RM>, (unsigned)grid, 256, 0, s, labels, n_docs, removed);
     return cudaGetLastError();
+}
+
+cudaError_t launch_lsh_clusters(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels, const uint32_t *removed,
+                                int sm_count, cudaStream_t s) {
+    if (n_docs <= 0) return cudaSuccess;
+    if (removed) return launch_clusters_t<true>(ix, n_docs, min_count, labels, removed, sm_count, s);
+    return launch_clusters_t<false>(ix, n_docs, min_count, labels, nullptr, sm_count, s);
+}
+
+}  // namespace dsk
+
+// ---- removal and compaction ---------------------------------------------------------------------------------------------
+// MinHashLSH.remove (lsh.py:509-528) drops a key from its buckets.  Here a removal only sets the document's bit in the
+// handle's bitmap (cap_docs bits, 1.25 MB at 10M documents: L2-resident), and the walks above skip it.  Compaction then
+// renumbers the remaining documents 0..m-1 in their old order, moves their rows down inside the index's own storage and
+// rebuilds the bucket tables from them, which gives the capacity back.
+namespace dsk {
+
+#ifdef DSK_EMU
+inline void atomic_add_i64(int64_t *p, int64_t v) { __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
+#else
+__device__ __forceinline__ void atomic_add_i64(int64_t *p, int64_t v) {
+    atomicAdd(reinterpret_cast<unsigned long long *>(p), (unsigned long long)v);
+}
+#endif
+
+// thread <-> listed id.  status[0] += ids outside [0, n_docs), status[1] += ids whose bit was set already (a repeat within
+// docs counts once: one of the atomicOr's sees the bit clear).  The loop runs over whole warps, so that every lane takes part
+// in the ballots that aggregate the counts before lane 0's atomicAdd.
+__global__ void __launch_bounds__(256) lsh_remove_kernel(uint32_t *removed, const int32_t *__restrict__ docs, int64_t n,
+                                                         int64_t n_docs, int64_t *status) {
+    const int lane = threadIdx.x & 31;
+    const int64_t n_up = (n + 31) & ~(int64_t)31;
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n_up; j += (int64_t)gridDim.x * blockDim.x) {
+        bool bad = false, again = false;
+        if (j < n) {
+            const int32_t d = docs[j];
+            if (d < 0 || d >= n_docs) {
+                bad = true;
+            } else {
+                const uint32_t bit = 1u << (d & 31);
+                again = (atomicOr(removed + (d >> 5), bit) & bit) != 0u;
+            }
+        }
+        const unsigned nb = __ballot_sync(0xFFFFFFFFu, bad), na = __ballot_sync(0xFFFFFFFFu, again);
+        if (lane == 0 && nb) atomic_add_i64(status, __popc(nb));
+        if (lane == 0 && na) atomic_add_i64(status + 1, __popc(na));
+    }
+}
+
+// out[j] = 1 iff docs[j] is in [0, n_docs) and not removed (removed == nullptr: nothing was)
+__global__ void __launch_bounds__(256) lsh_alive_kernel(const uint32_t *__restrict__ removed, const int32_t *__restrict__ docs,
+                                                        int64_t n, int64_t n_docs, uint8_t *__restrict__ out) {
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+        const int32_t d = docs[j];
+        out[j] = d >= 0 && d < n_docs && !(removed && is_removed(removed, d));
+    }
+}
+
+// surviving bits of bitmap word w among documents 0..n_docs-1
+__device__ __forceinline__ uint32_t alive_bits(const uint32_t *removed, int64_t w, int64_t n_docs) {
+    const int64_t left = n_docs - w * 32;
+    const uint32_t valid = left >= 32 ? 0xFFFFFFFFu : (1u << left) - 1u;
+    return ~removed[w] & valid;
+}
+
+__global__ void __launch_bounds__(256) compact_count_kernel(const uint32_t *__restrict__ removed, int64_t n_words,
+                                                            int64_t n_docs, int64_t *__restrict__ word_cnt) {
+    for (int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < n_words; w += (int64_t)gridDim.x * blockDim.x)
+        word_cnt[w] = __popc(alive_bits(removed, w, n_docs));
+}
+
+// remap[i] = new number of i (word prefix + surviving bits below i), -1 if removed; new2old[remap[i]] = i
+__global__ void __launch_bounds__(256) compact_remap_kernel(const uint32_t *__restrict__ removed, int64_t n_docs,
+                                                            const int64_t *__restrict__ word_ptr, int32_t *__restrict__ remap,
+                                                            int32_t *__restrict__ new2old) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_docs; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t w = i >> 5;
+        const int bit = (int)(i & 31);
+        const uint32_t alive = alive_bits(removed, w, n_docs);
+        if ((alive >> bit) & 1u) {
+            const int32_t t = (int32_t)(word_ptr[w] + __popc(alive & ((1u << bit) - 1u)));
+            remap[i] = t;
+            new2old[t] = (int32_t)i;
+        } else {
+            remap[i] = -1;
+        }
+    }
+}
+
+// warp <-> new number t in [a, b): stage[(t - a) * k ...] = row new2old[t]
+__global__ void __launch_bounds__(256) compact_gather_kernel(const uint32_t *__restrict__ sig, int k,
+                                                             const int32_t *__restrict__ new2old, int64_t a, int64_t b,
+                                                             uint32_t *__restrict__ stage) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    for (int64_t t = a + (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); t < b; t += warps) {
+        const uint32_t *src = sig + (int64_t)new2old[t] * k;
+        uint32_t *dst = stage + (t - a) * k;
+        for (int w = lane; w < k; w += 32) dst[w] = src[w];
+    }
+}
+
+constexpr size_t kCompactStageBytes = (size_t)64 << 20;   // rows moved per chunk of the compaction
+
+static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+static int64_t compact_stage_rows(int64_t n_docs, int k) {
+    int64_t rows = (int64_t)(kCompactStageBytes / ((size_t)k * 4));
+    if (rows < 1) rows = 1;
+    return rows < n_docs ? rows : n_docs;
+}
+
+// word counts int64[n_words] | word prefix int64[n_words + 1] | scan scratch int64[n_words / 1024 + 2] | new -> old
+// int32[n_docs] | row staging (at most kCompactStageBytes): nothing that grows as n_docs * k
+size_t lsh_compact_workspace_bytes(int64_t n_docs, int k) {
+    if (n_docs <= 0) return 0;
+    const int64_t n_words = (n_docs + 31) / 32;
+    return align256(n_words * 8) + align256((n_words + 1) * 8) + align256((n_words / 1024 + 2) * 8) +
+           align256((size_t)n_docs * 4) + align256((size_t)compact_stage_rows(n_docs, k) * k * 4);
+}
+
+cudaError_t launch_lsh_remove(uint32_t *removed, const int32_t *docs, int64_t n, int64_t n_docs, int64_t *status,
+                              int sm_count, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    int64_t grid = (n + 255) / 256;
+    if (grid > (int64_t)sm_count * 8) grid = (int64_t)sm_count * 8;
+    DSK_LAUNCH(lsh_remove_kernel, (unsigned)grid, 256, 0, s, removed, docs, n, n_docs, status);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_lsh_alive(const uint32_t *removed, const int32_t *docs, int64_t n, int64_t n_docs, uint8_t *out,
+                             int sm_count, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    int64_t grid = (n + 255) / 256;
+    if (grid > (int64_t)sm_count * 8) grid = (int64_t)sm_count * 8;
+    DSK_LAUNCH(lsh_alive_kernel, (unsigned)grid, 256, 0, s, removed, docs, n, n_docs, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_lsh_identity(int32_t *remap, int64_t n, int sm_count, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    int64_t grid = (n + 255) / 256;
+    if (grid > (int64_t)sm_count * 8) grid = (int64_t)sm_count * 8;
+    DSK_LAUNCH(uf_init_kernel, (unsigned)grid, 256, 0, s, remap, n);
+    return cudaGetLastError();
+}
+
+// Compacts the first n_docs documents of ix by the bitmap `removed`: remap[i] = new number or -1, *m = the number of
+// remaining documents.  Synchronises s once, to read m.  The caller then clears the bitmap and sets its n_docs to m.
+cudaError_t lsh_compact(const LshDev &ix, const uint32_t *removed, int64_t n_docs, int32_t *remap, void *ws, int64_t *m,
+                        int sm_count, cudaStream_t s) {
+    const int64_t n_words = (n_docs + 31) / 32;
+    char *p = static_cast<char *>(ws);
+    int64_t *word_cnt = reinterpret_cast<int64_t *>(p);
+    p += align256(n_words * 8);
+    int64_t *word_ptr = reinterpret_cast<int64_t *>(p);
+    p += align256((n_words + 1) * 8);
+    int64_t *scratch = reinterpret_cast<int64_t *>(p);
+    p += align256((n_words / 1024 + 2) * 8);
+    int32_t *new2old = reinterpret_cast<int32_t *>(p);
+    p += align256((size_t)n_docs * 4);
+    uint32_t *stage = reinterpret_cast<uint32_t *>(p);
+    const int64_t stage_rows = compact_stage_rows(n_docs, ix.k);
+    auto grid_of = [&](int64_t work) {
+        int64_t g = (work + 255) / 256;
+        return (unsigned)(g > (int64_t)sm_count * 8 ? (int64_t)sm_count * 8 : (g < 1 ? 1 : g));
+    };
+    DSK_LAUNCH(compact_count_kernel, grid_of(n_words), 256, 0, s, removed, n_words, n_docs, word_cnt);
+    cudaError_t e = launch_exclusive_scan(word_cnt, n_words, word_ptr, scratch, s);
+    if (e != cudaSuccess) return e;
+    DSK_LAUNCH(compact_remap_kernel, grid_of(n_docs), 256, 0, s, removed, n_docs, word_ptr, remap, new2old);
+    e = cudaMemcpyAsync(m, word_ptr + n_words, sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess || *m == n_docs) return e;   // nothing was removed: rows and tables stay as they are
+    // Move the rows in place, a chunk of new numbers [a, b) at a time: gather the chunk's source rows into the staging area,
+    // then write them to rows [a, b).  Safe because new numbers keep the old order: the source row s of new number t has
+    // s >= t >= a, the earlier chunks wrote only rows < a, and every later chunk's sources are rows >= b.
+    for (int64_t a = 0; a < *m; a += stage_rows) {
+        const int64_t b = a + stage_rows < *m ? a + stage_rows : *m;
+        DSK_LAUNCH(compact_gather_kernel, grid_of((b - a) * 32), 256, 0, s, ix.sig, ix.k, new2old, a, b, stage);
+        e = cudaMemcpyAsync(ix.sig + a * ix.k, stage, (size_t)(b - a) * ix.k * 4, cudaMemcpyDeviceToDevice, s);
+        if (e != cudaSuccess) return e;
+    }
+    // empty tables (as dsk_lsh_create leaves them), then rows 0..m-1 re-inserted from the index's own storage
+    e = cudaMemsetAsync(ix.slots, 0xFF, (size_t)ix.b * ix.cap_slots * 2 * sizeof(uint64_t), s);
+    if (e == cudaSuccess) e = launch_lsh_insert(ix, ix.sig, 0, *m, sm_count, s);
+    return e;
 }
 
 }  // namespace dsk

@@ -663,6 +663,87 @@ class GpuLSH:
             labels = labels[:n]
         return labels.cpu().numpy() if to_host else labels
 
+    # -- removal and compaction (MinHashLSH.remove, lsh.py:497-528) ----------------------------------------------------
+    def _doc_tensor(self, docs):
+        """``docs`` (one number, a sequence, a numpy array or a CUDA tensor) as a 1-D int64 CUDA tensor."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        if isinstance(docs, torch.Tensor):
+            if docs.is_floating_point() or docs.is_complex() or docs.dtype == torch.bool:
+                raise TypeError("document numbers must be integers")
+            return docs.reshape(-1).to(device=dev, dtype=torch.int64)
+        a = np.asarray(docs).reshape(-1)
+        if a.size and a.dtype.kind not in "iu":
+            raise TypeError("document numbers must be integers")
+        return torch.from_numpy(a.astype(np.int64)).to(dev)
+
+    def remove(self, docs) -> None:
+        """Remove documents (their numbers: one, a sequence, a numpy array or a CUDA tensor) from the index, as
+        ``MinHashLSH.remove`` removes keys.  Afterwards ``query`` never returns them, ``candidate_pairs`` pairs nothing
+        with them (their own rows are empty) and ``duplicate_clusters`` labels them -1; the pairs and clusters of the
+        remaining documents are those before the removal restricted to them.
+
+        Document numbers do not change until ``compact()``, and ``len()`` still counts removed documents until then.
+        Raises ``ValueError("The given key does not exist")`` if a number is out of range, already removed or listed twice;
+        the index is then unchanged (everything is checked before anything is removed)."""
+        import torch
+        d = self._doc_tensor(docs)
+        n = len(self)
+        if d.numel() == 0:
+            return
+        if bool(((d < 0) | (d >= n)).any()) or torch.unique(d).numel() != d.numel():
+            raise ValueError("The given key does not exist")
+        d32 = d.to(torch.int32)
+        if not bool(self._alive(d32).all()):
+            raise ValueError("The given key does not exist")
+        with torch.cuda.device(self.device):
+            status = torch.zeros((2,), dtype=torch.int64, device=d32.device)
+            nv.check(nv.load().dsk_lsh_remove(self._h, d32.data_ptr(), d32.numel(), status.data_ptr(),
+                                              torch.cuda.current_stream().cuda_stream))
+
+    def _alive(self, d32):
+        import torch
+        with torch.cuda.device(self.device):
+            out = torch.empty((max(d32.numel(), 1),), dtype=torch.uint8, device=d32.device)
+            nv.check(nv.load().dsk_lsh_alive(self._h, d32.data_ptr(), d32.numel(), out.data_ptr(),
+                                             torch.cuda.current_stream().cuda_stream))
+        return out[:d32.numel()].bool()
+
+    def alive(self, docs=None, to_host: bool = True):
+        """Bool mask: True where the document number is in ``[0, len(self))`` and not removed.  Over ``docs``, or over all
+        ``len(self)`` numbers when ``docs`` is None."""
+        import torch
+        if docs is None:
+            d32 = torch.arange(len(self), dtype=torch.int32, device=torch.device("cuda", self.device))
+        else:
+            d = self._doc_tensor(docs)
+            d32 = torch.where((d >= 0) & (d < (1 << 31)), d, torch.full_like(d, -1)).to(torch.int32)
+        mask = self._alive(d32)
+        return mask.cpu().numpy() if to_host else mask
+
+    def compact(self, to_host: bool = True):
+        """Renumber the remaining documents ``0..m-1`` in their old order, rebuild the buckets from them and free the
+        capacity the removed ones held.  Returns ``remap`` (int32, one entry per old number: the new number, or -1 for a
+        removed document).  Because the order is kept, ``candidate_pairs`` afterwards equals the earlier pairs mapped
+        through ``remap``, ``duplicate_clusters`` equals ``remap[labels_before]`` on the remaining documents, and the
+        index behaves as a fresh ``GpuLSH`` into which the remaining rows were inserted in order.  ``keys``, when it
+        holds one key per document, keeps the remaining keys.  Waits for the device once."""
+        import torch
+        n = len(self)
+        lib = nv.load()
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.device(self.device):
+            ws_bytes = int(lib.dsk_lsh_compact_workspace_size(self._h))
+            ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
+            remap = torch.empty((max(n, 1),), dtype=torch.int32, device=dev)
+            nv.check(lib.dsk_lsh_compact(self._h, remap.data_ptr(), ws.data_ptr(), ws_bytes,
+                                         torch.cuda.current_stream().cuda_stream))
+            remap = remap[:n]
+        if self.keys and len(self.keys) == n:
+            keep = remap.cpu().numpy() >= 0
+            self.keys = [k for k, kept in zip(self.keys, keep) if kept]
+        return remap.cpu().numpy() if to_host else remap
+
 
 def _jaccard_min_count(min_jaccard: Optional[float], num_perm: int) -> int:
     """The smallest count c in 0..num_perm with ``float(c) / float(num_perm) >= min_jaccard`` -- exactly the pairs

@@ -232,7 +232,24 @@ DSK_API int dsk_wmh_minhash(const dsk_wmh *g, const float *d_v, int64_t n, int64
  *   dsk_lsh_clusters     d_labels[i] = smallest document number of i's connected component of the kept pairs' graph
  *                        (deterministic; d_labels is the union-find's parent array, no other workspace).  min_count = 0
  *                        links each document to the first equal member of each of its buckets: linear in the index.
- *                        min_count > 0 walks every pair: quadratic in the size of each bucket. */
+ *                        min_count > 0 walks every pair: quadratic in the size of each bucket.
+ * Removal (MinHashLSH.remove, lsh.py:509-528).  A removed document keeps its number until dsk_lsh_compact, and n_docs
+ * (dsk_lsh_size) still counts it.  query never returns it, the self-join pairs nothing with it (its own count is 0) and
+ * dsk_lsh_clusters labels it -1; pairs among the remaining documents are exactly those before the removal.  An index that
+ * never removed anything, or whose removals were compacted, runs the same kernels as before removal existed.
+ *   dsk_lsh_remove       marks the n documents d_docs[0..n) removed (asynchronous, ordered on the stream; the first call
+ *                        allocates a bitmap of capacity_docs bits).  d_status[0] += ids outside [0, n_docs), which are
+ *                        ignored; d_status[1] += ids already removed, a repeat within d_docs included.  Idempotent.
+ *   dsk_lsh_alive        d_out[j] = 1 iff d_docs[j] is in [0, n_docs) and not removed, else 0
+ *   dsk_lsh_compact      renumbers the remaining documents 0..m-1 in their old order and rebuilds the bucket tables from
+ *                        them: d_remap[old] = new number, or -1 for a removed document (n_docs entries).  The rows move
+ *                        inside the index's own storage, so the freed capacity can be inserted again.  Afterwards the index
+ *                        behaves as a fresh one into which the remaining rows were inserted in order.  The call
+ *                        SYNCHRONISES the stream once, to read m, and then sets n_docs = m; with nothing removed since
+ *                        the last compaction it writes the identity remap and returns without synchronising.
+ *   dsk_lsh_compact_workspace_size  bytes of d_ws (16-byte aligned) for the index's current n_docs: the removal bitmap's
+ *                        per-word prefix counts, the new -> old index (int32 per document) and a fixed staging area of
+ *                        at most 64 MB for the rows.  It does not grow as n_docs * num_perm. */
 typedef struct dsk_lsh dsk_lsh;
 DSK_API int dsk_lsh_create(int num_perm, int b, int r, int64_t capacity_docs, int device, dsk_lsh **out);
 DSK_API void dsk_lsh_destroy(dsk_lsh *ix);
@@ -248,6 +265,10 @@ DSK_API int dsk_lsh_pairs_count(const dsk_lsh *ix, int min_count, int64_t *d_cou
 DSK_API int dsk_lsh_pairs_fill(const dsk_lsh *ix, int min_count, const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq,
                                void *stream);
 DSK_API int dsk_lsh_clusters(const dsk_lsh *ix, int min_count, int32_t *d_labels, void *stream);
+DSK_API int dsk_lsh_remove(dsk_lsh *ix, const int32_t *d_docs, int64_t n, int64_t *d_status, void *stream);
+DSK_API int dsk_lsh_alive(const dsk_lsh *ix, const int32_t *d_docs, int64_t n, uint8_t *d_out, void *stream);
+DSK_API size_t dsk_lsh_compact_workspace_size(const dsk_lsh *ix);
+DSK_API int dsk_lsh_compact(dsk_lsh *ix, int32_t *d_remap, void *d_ws, size_t ws_bytes, void *stream);
 
 /* ---- Jaccard estimate -----------------------------------------------------------------------
  * d_count[p] = number of positions where rows d_i[p] and d_j[p] of the [n_rows, num_perm] u32

@@ -32,9 +32,10 @@ def ev_time(fn, iters=3, warm=1):
     return e0.elapsed_time(e1) / iters
 
 
-def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False):
+def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, remove_leg=False):
     """10M x 128 tokens, K=256 + LSH(0.8) insert + query (here n_docs on one GPU).  dedup_leg: also the self-join of
-    the index (candidate_pairs, duplicate_clusters with and without min_jaccard=0.8) against the host flow it replaces."""
+    the index (candidate_pairs, duplicate_clusters with and without min_jaccard=0.8) against the host flow it replaces.
+    remove_leg: also removal of the duplicates from the index and its compaction (c3_remove)."""
     perms = _make_permutations(k, 1)
     g = torch.Generator(device="cuda").manual_seed(3)
     tok = torch.randint(-2 ** 31, 2 ** 31 - 1, (n_docs, t), dtype=torch.int32, device="cuda", generator=g)
@@ -100,6 +101,8 @@ def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False):
         ref.query(row)
     cpu_q = (time.perf_counter() - t0) / 5000
     dedup = c3_dedup(lsh, src, dst, ref, hs) if dedup_leg else {}
+    if remove_leg:
+        dedup.update(c3_remove(lsh, sig, q))
     return {"config": "C3 (1 GPU)", "docs": n_docs, "tokens": t, "num_perm": k, "b": lsh.b, "r": lsh.r,
             "signature_ms": ms_sig, "signatures_per_s": n_docs / ms_sig * 1e3,
             "lsh_insert_ms": ms_ins, "lsh_insert_docs_per_s": n_docs / ms_ins * 1e3,
@@ -142,6 +145,68 @@ def c3_dedup(lsh, src, dst, ref, hs, min_jaccard=0.8):
     ns = len(hs)
     connected_components(coo_matrix((np.ones(len(ii)), (ii, dd)), shape=(ns, ns)), directed=False)
     out["dedup_host_flow_us_per_doc"] = (time.perf_counter() - t0) / ns * 1e6
+    return out
+
+
+def c3_remove(lsh, sig, q, min_jaccard=0.8, rounds=3):
+    """GpuLSH.remove of the non-root documents of duplicate_clusters(min_jaccard), then the walks with removals present,
+    then compact().  The removals go to a second index of the same rows, so that the calls without removals (``lsh``, the
+    kernels that run when nothing was removed) and with them (the removal-aware kernels) alternate in one process: each
+    round times every call on both indexes with CUDA events (3 calls after 1 warm-up call).  remove() and compact() run
+    once each, so they are timed once: both wait for the device inside (remove() checks its ids first, compact() reads
+    the number of remaining documents), and the events span the whole call."""
+    n, k = len(lsh), lsh.h
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    rm = dsk.GpuLSH(threshold=0.8, num_perm=k, capacity=n)
+    torch.cuda.synchronize()
+    e0.record()
+    rm.insert(sig)
+    e1.record()
+    torch.cuda.synchronize()
+    ms_insert = e0.elapsed_time(e1)
+    labels = rm.duplicate_clusters(min_jaccard, to_host=False)
+    gone = torch.nonzero(labels != torch.arange(n, dtype=torch.int32, device="cuda")).view(-1)
+    small = dsk.GpuLSH(threshold=0.8, num_perm=k, capacity=64)   # first launch of the remove / alive kernels: not timed
+    small.insert(sig[:64])
+    small.remove([1, 2])
+    del small
+    torch.cuda.synchronize()
+    e0.record()
+    rm.remove(gone)
+    e1.record()
+    torch.cuda.synchronize()
+    ms_remove = e0.elapsed_time(e1)
+    calls = {"query": lambda ix: ix.query(q, to_host=False),
+             "candidate_pairs": lambda ix: ix.candidate_pairs(to_host=False),
+             "duplicate_clusters": lambda ix: ix.duplicate_clusters(to_host=False),
+             "duplicate_clusters_min_jaccard": lambda ix: ix.duplicate_clusters(min_jaccard, to_host=False)}
+    times = {name: {"without": [], "with": []} for name in calls}
+    for _ in range(rounds):
+        for name, fn in calls.items():
+            times[name]["without"].append(ev_time(lambda: fn(lsh)))
+            times[name]["with"].append(ev_time(lambda: fn(rm)))
+    p0, x0, _ = lsh.candidate_pairs(to_host=False)
+    rows0 = torch.repeat_interleave(torch.arange(n, device="cuda"), p0[1:] - p0[:-1])
+    alive = rm.alive(to_host=False)
+    kept_pairs = int((alive[rows0] & alive[x0.long()]).sum().item())
+    p1, _, _ = rm.candidate_pairs(to_host=False)
+    torch.cuda.synchronize()
+    e0.record()
+    remap = rm.compact(to_host=False)
+    e1.record()
+    torch.cuda.synchronize()
+    ms_compact = e0.elapsed_time(e1)
+    ms_pairs_after = ev_time(lambda: rm.candidate_pairs(to_host=False))
+    p2, _, _ = rm.candidate_pairs(to_host=False)
+    out = {"remove_min_jaccard": min_jaccard, "remove_docs": int(gone.numel()), "remove_ms_once": ms_remove,
+           "remove_second_index_insert_ms": ms_insert, "remove_docs_remaining": len(rm),
+           "remove_pairs_before": int(p0[-1].item()), "remove_pairs_with_removals": int(p1[-1].item()),
+           "remove_pairs_among_remaining_before": kept_pairs, "remove_pairs_after_compact": int(p2[-1].item()),
+           "remove_remap_monotone": bool((remap[remap >= 0].diff() == 1).all().item()),
+           "remove_compact_ms_once": ms_compact, "remove_candidate_pairs_after_compact_ms": ms_pairs_after}
+    for name, t in times.items():
+        out["remove_%s_ms_without_removals" % name] = t["without"]
+        out["remove_%s_ms_with_removals" % name] = t["with"]
     return out
 
 
@@ -216,9 +281,12 @@ if __name__ == "__main__":
                     help="also time GpuLSH.insert_tokens (fused signatures + insert); tools/diag_fused.py times it alone")
     ap.add_argument("--c3-dedup", action="store_true",
                     help="also time GpuLSH.candidate_pairs / duplicate_clusters on the C3 index and the host flow they replace")
+    ap.add_argument("--c3-remove", action="store_true",
+                    help="after the dedup leg: GpuLSH.remove of the duplicates, the walks with removals present beside the "
+                         "same calls without removals, and compact()")
     a = ap.parse_args()
     if a.c3_docs > 0:
-        print(json.dumps(c3(a.c3_docs, fused_leg=a.c3_fused, dedup_leg=a.c3_dedup)), flush=True)
+        print(json.dumps(c3(a.c3_docs, fused_leg=a.c3_fused, dedup_leg=a.c3_dedup, remove_leg=a.c3_remove)), flush=True)
     for fn, arg in ((c4, a.c4_vecs), (c5, a.c5_rows)):
         if arg > 0:
             print(json.dumps(fn(arg)), flush=True)
