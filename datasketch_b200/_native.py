@@ -61,6 +61,9 @@ SIGNATURES = {
     "dsk_lsh_pairs_count": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "dsk_lsh_pairs_fill": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dsk_lsh_clusters": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "dsk_lsh_query_jaccard_count": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
+    "dsk_lsh_query_jaccard_fill": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dsk_lsh_query_best": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
     "dsk_lsh_remove": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "dsk_lsh_alive": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "dsk_lsh_compact_workspace_size": (ctypes.c_size_t, [c_void_p]),

@@ -886,6 +886,55 @@ int dsk_lsh_clusters(const dsk_lsh *ix, int min_count, int32_t *d_labels, void *
     return DSK_OK;
 }
 
+// handle, min_count in [0, num_perm], nq >= 0 and, when nq > 0, the query matrix and every output buffer
+static int check_query_pairs(const char *who, const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count,
+                             bool bufs) {
+    int rc = check_self_join(who, ix, min_count);
+    if (rc) return rc;
+    if (nq < 0) {
+        set_error("%s: nq must be >= 0 (got %lld)", who, (long long)nq);
+        return DSK_ERR_INVALID;
+    }
+    if (nq > 0 && (!d_qsig || !bufs)) {
+        set_error("%s: null buffer", who);
+        return DSK_ERR_INVALID;
+    }
+    return DSK_OK;
+}
+
+static int run_query_pairs(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, int64_t *d_counts,
+                           const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq, void *stream) {
+    if (nq == 0) return DSK_OK;
+    DevInfo *dev;
+    int rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    DSK_CUDA(launch_lsh_query_pairs(ix->dev, d_qsig, nq, ix->n_docs, min_count, d_counts, d_ptr, d_idx, d_eq,
+                                    ix->walk_bitmap(), dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_lsh_query_jaccard_count(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, int64_t *d_counts,
+                                void *stream) {
+    int rc = check_query_pairs("dsk_lsh_query_jaccard_count", ix, d_qsig, nq, min_count, d_counts != nullptr);
+    if (rc) return rc;
+    return run_query_pairs(ix, d_qsig, nq, min_count, d_counts, nullptr, nullptr, nullptr, stream);
+}
+
+int dsk_lsh_query_jaccard_fill(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, const int64_t *d_ptr,
+                               int32_t *d_idx, int32_t *d_eq, void *stream) {
+    int rc = check_query_pairs("dsk_lsh_query_jaccard_fill", ix, d_qsig, nq, min_count, d_ptr && d_idx && d_eq);
+    if (rc) return rc;
+    return run_query_pairs(ix, d_qsig, nq, min_count, nullptr, d_ptr, d_idx, d_eq, stream);
+}
+
+int dsk_lsh_query_best(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, int32_t *d_idx, int32_t *d_eq,
+                       void *stream) {
+    int rc = check_query_pairs("dsk_lsh_query_best", ix, d_qsig, nq, min_count, d_idx && d_eq);
+    if (rc) return rc;
+    return run_query_pairs(ix, d_qsig, nq, min_count, nullptr, nullptr, d_idx, d_eq, stream);
+}
+
 static int check_ids(const char *who, const dsk_lsh *ix, const void *d_docs, int64_t n, const void *d_out) {
     if (!ix) {
         set_error("%s: null handle", who);

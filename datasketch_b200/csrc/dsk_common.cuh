@@ -135,6 +135,12 @@ cudaError_t launch_lsh_pairs(const LshDev &ix, int64_t n_docs, int min_count, in
                              int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s);
 cudaError_t launch_lsh_clusters(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels, const uint32_t *removed,
                                 int sm_count, cudaStream_t s);
+// the self-join's walk for nq query rows outside the index (every d < n_docs eligible): per-query counts of the kept
+// candidates; the fill of idx / eq at ptr[q] (counts == nullptr); or each query's best kept candidate at idx[q] / eq[q]
+// (counts == ptr == nullptr)
+cudaError_t launch_lsh_query_pairs(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count,
+                                   int64_t *counts, const int64_t *ptr, int32_t *idx, int32_t *eq, const uint32_t *removed,
+                                   int sm_count, cudaStream_t s);
 // removal (bits of the bitmap) and compaction of the index
 cudaError_t launch_lsh_remove(uint32_t *removed, const int32_t *docs, int64_t n, int64_t n_docs, int64_t *status,
                               int sm_count, cudaStream_t s);

@@ -371,7 +371,7 @@ __global__ void __launch_bounds__(256) uf_flatten_kernel(int32_t *labels, int64_
     }
 }
 
-enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2 };
+enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2, QUERY_COUNT = 3, QUERY_FILL = 4, QUERY_BEST = 5 };
 
 // warp <-> document i, lane <-> band (bands beyond 32 in further rounds), row i staged once in shared memory.  Each lane
 // probes its band's table with the fingerprint of i's own tuple and walks the bucket's chain to its next partner d: d < i,
@@ -383,24 +383,35 @@ enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2 };
 //   PAIRS_UNION  united with i in labels[] (nothing materialised)
 // RM: a removed i has no partners (its whole iteration is skipped, warp-uniformly; PAIRS_COUNT still writes counts[i] = 0),
 // and a removed d is no partner.
+// The QUERY modes run the same walk for the nq rows of qsig, which are not in the index: row i is qsig + i * k, and every
+// document d < n_docs is eligible (the bound of lsh_query_kernel), so the partners of query i are exactly query(row i):
+//   QUERY_COUNT  counts[i] = number kept
+//   QUERY_FILL   written at idx / eq [ptr[i] ...), in no particular order
+//   QUERY_BEST   idx[i] / eq[i] = the kept partner with the largest eq, the smallest d among equal ones (-1 / -1: none).
+//                Each lane keeps its own best and a warp shuffle reduction picks the query's: no atomics.
+// In the PAIRS modes qsig and nq are unused and the code is the self-join's alone.
 template <int MODE, bool RM>
 __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t n_docs, int min_count,
                                                         int64_t *__restrict__ counts, const int64_t *__restrict__ ptr,
                                                         int32_t *__restrict__ out_idx, int32_t *__restrict__ out_eq,
-                                                        int32_t *labels, const uint32_t *__restrict__ removed) {
+                                                        int32_t *labels, const uint32_t *__restrict__ removed,
+                                                        const uint32_t *__restrict__ qsig, int64_t nq) {
+    constexpr bool QUERY = MODE >= QUERY_COUNT;
     DSK_DYNAMIC_SMEM_T(uint32_t, s_rows, 16);   // [warps][k]
     const int lane = threadIdx.x & 31;
     uint32_t *row = s_rows + (int64_t)(threadIdx.x >> 5) * ix.k;
     const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
     const uint64_t mask = (uint64_t)ix.cap_slots - 1;
-    const bool need_eq = MODE == PAIRS_FILL || min_count > 0;
+    const bool need_eq = MODE == PAIRS_FILL || MODE == QUERY_FILL || MODE == QUERY_BEST || min_count > 0;
     const unsigned below = (1u << lane) - 1u;
-    for (int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < n_docs; i += warps) {
-        if (RM && is_removed(removed, i)) {
+    for (int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < (QUERY ? nq : n_docs); i += warps) {
+        if (!QUERY && RM && is_removed(removed, i)) {
             if (MODE == PAIRS_COUNT && lane == 0) counts[i] = 0;
             continue;
         }
-        const uint32_t *irow = ix.sig + i * ix.k;
+        const int64_t bound = QUERY ? n_docs : i;   // partners d < bound
+        int32_t best_d = -1, best_eq = -1;          // QUERY_BEST: this lane's best kept partner
+        const uint32_t *irow = (QUERY ? qsig : ix.sig) + i * ix.k;
         __syncwarp();
         for (int w = lane; w < ix.k; w += 32) row[w] = irow[w];
         __syncwarp();
@@ -425,7 +436,7 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
                 while (d >= 0) {
                     const int32_t cur = d;
                     d = ix.next[(int64_t)cur * ix.b + band];
-                    if (cur < i && !(RM && is_removed(removed, cur))) {
+                    if (cur < bound && !(RM && is_removed(removed, cur))) {
                         const uint32_t *drow = ix.sig + (int64_t)cur * ix.k;
                         if (tuple_eq(drow + band * ix.r, it, ix.r)) {
                             bool dup = false;
@@ -452,9 +463,11 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
                 const bool keep = cand >= 0 && eq >= min_count;
                 if (MODE == PAIRS_UNION) {
                     if (keep) uf_union(labels, (int32_t)i, cand);
+                } else if (MODE == QUERY_BEST) {
+                    if (keep && (eq > best_eq || (eq == best_eq && cand < best_d))) { best_eq = eq; best_d = cand; }
                 } else {
                     const unsigned kept = __ballot_sync(0xFFFFFFFFu, keep);
-                    if (MODE == PAIRS_FILL && keep) {
+                    if ((MODE == PAIRS_FILL || MODE == QUERY_FILL) && keep) {
                         const int64_t pos = ptr[i] + total + __popc(kept & below);
                         out_idx[pos] = cand;
                         out_eq[pos] = eq;
@@ -463,7 +476,15 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
                 }
             }
         }
-        if (MODE == PAIRS_COUNT && lane == 0) counts[i] = total;
+        if ((MODE == PAIRS_COUNT || MODE == QUERY_COUNT) && lane == 0) counts[i] = total;
+        if (MODE == QUERY_BEST) {   // largest eq, then smallest d; a lane without a kept partner holds (-1, -1) and loses
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const int32_t oe = __shfl_xor_sync(0xFFFFFFFFu, best_eq, o), od = __shfl_xor_sync(0xFFFFFFFFu, best_d, o);
+                if (oe > best_eq || (oe == best_eq && od < best_d)) { best_eq = oe; best_d = od; }
+            }
+            if (lane == 0) { out_idx[i] = best_d; out_eq[i] = best_eq; }
+        }
     }
 }
 
@@ -504,21 +525,22 @@ __global__ void __launch_bounds__(256) lsh_link_kernel(const LshDev ix, int64_t 
     }
 }
 
-// the pair walk's launch shape: up to 8 warps per CTA, each with a K-word row in shared memory
-template <bool RM>
-static cudaError_t pairs_shape(const LshDev &ix, int64_t n_docs, int sm_count, int *warps, unsigned *grid, size_t *smem) {
+// the pair walk's launch shape for `rows` staged rows (documents, or queries with M0 = QUERY_COUNT): up to 8 warps per
+// CTA, each with a K-word row in shared memory.  Allows that much shared memory to the modes M0, M0 + 1 and M0 + 2.
+template <bool RM, int M0 = PAIRS_COUNT>
+static cudaError_t pairs_shape(const LshDev &ix, int64_t rows, int sm_count, int *warps, unsigned *grid, size_t *smem) {
     int w = 8;
     while (w > 1 && (size_t)w * ix.k * 4 > 48 * 1024) w >>= 1;
     *warps = w;
     *smem = (size_t)w * ix.k * 4;
-    int64_t g = (n_docs + w - 1) / w;
+    int64_t g = (rows + w - 1) / w;
     if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
     *grid = (unsigned)g;
-    cudaError_t e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_COUNT, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+    cudaError_t e = cudaFuncSetAttribute(lsh_pairs_kernel<M0, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_FILL, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+        e = cudaFuncSetAttribute(lsh_pairs_kernel<M0 + 1, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(lsh_pairs_kernel<PAIRS_UNION, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+        e = cudaFuncSetAttribute(lsh_pairs_kernel<M0 + 2, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
     return e;
 }
 
@@ -532,10 +554,10 @@ static cudaError_t launch_pairs_t(const LshDev &ix, int64_t n_docs, int min_coun
     if (e != cudaSuccess) return e;
     if (counts)
         DSK_LAUNCH((lsh_pairs_kernel<PAIRS_COUNT, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr,
-                   nullptr, nullptr, nullptr, removed);
+                   nullptr, nullptr, nullptr, removed, nullptr, 0);
     else
         DSK_LAUNCH((lsh_pairs_kernel<PAIRS_FILL, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
-                   nullptr, removed);
+                   nullptr, removed, nullptr, 0);
     return cudaGetLastError();
 }
 
@@ -565,7 +587,7 @@ static cudaError_t launch_clusters_t(const LshDev &ix, int64_t n_docs, int min_c
         cudaError_t e = pairs_shape<RM>(ix, n_docs, sm_count, &warps, &pg, &smem);
         if (e != cudaSuccess) return e;
         DSK_LAUNCH((lsh_pairs_kernel<PAIRS_UNION, RM>), pg, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr,
-                   nullptr, nullptr, labels, removed);
+                   nullptr, nullptr, labels, removed, nullptr, 0);
     }
     DSK_LAUNCH(uf_flatten_kernel<RM>, (unsigned)grid, 256, 0, s, labels, n_docs, removed);
     return cudaGetLastError();
@@ -576,6 +598,38 @@ cudaError_t launch_lsh_clusters(const LshDev &ix, int64_t n_docs, int min_count,
     if (n_docs <= 0) return cudaSuccess;
     if (removed) return launch_clusters_t<true>(ix, n_docs, min_count, labels, removed, sm_count, s);
     return launch_clusters_t<false>(ix, n_docs, min_count, labels, nullptr, sm_count, s);
+}
+
+template <bool RM>
+static cudaError_t launch_query_pairs_t(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count,
+                                        int mode, int64_t *counts, const int64_t *ptr, int32_t *idx, int32_t *eq,
+                                        const uint32_t *removed, int sm_count, cudaStream_t s) {
+    int warps;
+    unsigned grid;
+    size_t smem;
+    cudaError_t e = pairs_shape<RM, QUERY_COUNT>(ix, nq, sm_count, &warps, &grid, &smem);
+    if (e != cudaSuccess) return e;
+    if (mode == QUERY_COUNT)
+        DSK_LAUNCH((lsh_pairs_kernel<QUERY_COUNT, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr,
+                   nullptr, nullptr, nullptr, removed, qsig, nq);
+    else if (mode == QUERY_FILL)
+        DSK_LAUNCH((lsh_pairs_kernel<QUERY_FILL, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
+                   nullptr, removed, qsig, nq);
+    else
+        DSK_LAUNCH((lsh_pairs_kernel<QUERY_BEST, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr, idx,
+                   eq, nullptr, removed, qsig, nq);
+    return cudaGetLastError();
+}
+
+// The pair walk for the nq rows of qsig against the index's first n_docs documents.  counts != nullptr: counts[q] of the
+// kept candidates; ptr != nullptr: the fill of idx / eq at ptr[q]; else idx[q] / eq[q] = q's best kept candidate.
+cudaError_t launch_lsh_query_pairs(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count,
+                                   int64_t *counts, const int64_t *ptr, int32_t *idx, int32_t *eq, const uint32_t *removed,
+                                   int sm_count, cudaStream_t s) {
+    if (nq <= 0) return cudaSuccess;
+    const int mode = counts ? QUERY_COUNT : ptr ? QUERY_FILL : QUERY_BEST;
+    if (removed) return launch_query_pairs_t<true>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, removed, sm_count, s);
+    return launch_query_pairs_t<false>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, nullptr, sm_count, s);
 }
 
 }  // namespace dsk

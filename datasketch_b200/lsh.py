@@ -616,6 +616,57 @@ class GpuLSH:
             out.append([self.keys[i] for i in ids] if self.keys else ids.tolist())
         return out
 
+    # -- queries verified on the device: Jaccard counts, a min_jaccard filter and each query's best match -------------
+    def query_jaccard(self, sig, min_jaccard: Optional[float] = None, to_host: bool = True):
+        """Candidates of every row of ``sig`` with their Jaccard counts: ``(ptr int64[Q+1], idx int32[M], eq int32[M])``.
+
+        ``idx[ptr[q]:ptr[q+1]]`` lists each candidate of query q once, in no particular order; without ``min_jaccard``
+        the candidates, as a set, are ``query(sig)``'s.  ``eq`` is the number of the ``num_perm`` positions where the query
+        row and the document's row agree, so ``eq / num_perm`` is ``MinHash.jaccard``.  ``min_jaccard`` keeps only the
+        candidates with ``MinHash.jaccard >= min_jaccard``: ``[d for d in lsh.query(m) if m.jaccard(doc[d]) >= t]`` for
+        every query at once, on the rows the index holds.  A query costs time linear in the size of the buckets it hits."""
+        import torch
+        mc = _jaccard_min_count(min_jaccard, self.h)
+        d_q = self._dev_sig(sig)
+        nq = d_q.shape[0]
+        dev = d_q.device
+        lib = nv.load()
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream().cuda_stream
+            counts = torch.empty((max(nq, 1),), dtype=torch.int64, device=dev)
+            ptr = torch.empty((nq + 1,), dtype=torch.int64, device=dev)
+            scratch = torch.empty((nq // 1024 + 2,), dtype=torch.int64, device=dev)
+            nv.check(lib.dsk_lsh_query_jaccard_count(self._h, d_q.data_ptr(), nq, mc, counts.data_ptr(), st))
+            nv.check(lib.dsk_exclusive_scan(counts.data_ptr(), nq, ptr.data_ptr(), scratch.data_ptr(), st))
+            total = int(ptr[nq].item())
+            idx = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
+            eq = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
+            nv.check(lib.dsk_lsh_query_jaccard_fill(self._h, d_q.data_ptr(), nq, mc, ptr.data_ptr(), idx.data_ptr(),
+                                                    eq.data_ptr(), st))
+            idx, eq = idx[:total], eq[:total]
+        if to_host:
+            return ptr.cpu().numpy(), idx.cpu().numpy(), eq.cpu().numpy()
+        return ptr, idx, eq
+
+    def query_best(self, sig, min_jaccard: Optional[float] = None, to_host: bool = True):
+        """Each query's closest indexed document: ``(idx int32[Q], eq int32[Q])``, the candidate of ``query_jaccard(sig,
+        min_jaccard)`` with the largest ``eq``, the smallest document number among equal ones.  Both are -1 where the
+        query keeps no candidate.  ``eq / num_perm`` is the query's largest ``MinHash.jaccard`` over its candidates, e.g. a
+        document's similarity to the corpus in a decontamination report.  One launch, without a host synchronisation."""
+        import torch
+        mc = _jaccard_min_count(min_jaccard, self.h)
+        d_q = self._dev_sig(sig)
+        nq = d_q.shape[0]
+        with torch.cuda.device(self.device):
+            idx = torch.empty((max(nq, 1),), dtype=torch.int32, device=d_q.device)
+            eq = torch.empty((max(nq, 1),), dtype=torch.int32, device=d_q.device)
+            nv.check(nv.load().dsk_lsh_query_best(self._h, d_q.data_ptr(), nq, mc, idx.data_ptr(), eq.data_ptr(),
+                                                  torch.cuda.current_stream().cuda_stream))
+            idx, eq = idx[:nq], eq[:nq]
+        if to_host:
+            return idx.cpu().numpy(), eq.cpu().numpy()
+        return idx, eq
+
     # -- self-join: near-duplicate pairs and clusters of the indexed documents ------------------------------------------
     def candidate_pairs(self, min_jaccard: Optional[float] = None, to_host: bool = True):
         """Every candidate pair among the ``n = len(self)`` indexed documents, once, as CSR arrays

@@ -265,6 +265,25 @@ DSK_API int dsk_lsh_pairs_count(const dsk_lsh *ix, int min_count, int64_t *d_cou
 DSK_API int dsk_lsh_pairs_fill(const dsk_lsh *ix, int min_count, const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq,
                                void *stream);
 DSK_API int dsk_lsh_clusters(const dsk_lsh *ix, int min_count, int32_t *d_labels, void *stream);
+/* Query rows that are NOT in the index, verified on the device (MinHashLSH.query + MinHash.jaccard per candidate,
+ * lsh.py:370-432, minhash.py:299-324): the self-join's walk with the query row staged in place of document i and every
+ * document d < n_docs eligible.  d_qsig is [nq, num_perm] u32; min_count in [0, num_perm] keeps the candidates with
+ * eq >= min_count, where eq = number of positions where the query row and the document's row agree.  Removed documents
+ * (since the last dsk_lsh_compact) are never returned.  nq == 0 with null buffers is a valid no-op.  A query that hits a
+ * bucket of s members reads up to s rows of num_perm words: its time is linear in the size of the buckets it hits.
+ *   dsk_lsh_query_jaccard_count  d_counts[q] = number of kept candidates of query q
+ *   dsk_lsh_query_jaccard_fill   after dsk_exclusive_scan of the counts: writes q's kept candidates (each once, unordered)
+ *                                at d_idx[d_ptr[q] .. d_ptr[q+1]) and their eq at the same positions of d_eq.  Without a
+ *                                filter the candidates are exactly dsk_lsh_query_fill's.
+ *   dsk_lsh_query_best           d_idx[q] / d_eq[q] = q's kept candidate with the largest eq, the smallest document number
+ *                                among equal ones (deterministic); -1 / -1 when q keeps none.  One launch: no count, scan
+ *                                or fill, no synchronisation. */
+DSK_API int dsk_lsh_query_jaccard_count(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count,
+                                        int64_t *d_counts, void *stream);
+DSK_API int dsk_lsh_query_jaccard_fill(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count,
+                                       const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq, void *stream);
+DSK_API int dsk_lsh_query_best(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, int32_t *d_idx,
+                               int32_t *d_eq, void *stream);
 DSK_API int dsk_lsh_remove(dsk_lsh *ix, const int32_t *d_docs, int64_t n, int64_t *d_status, void *stream);
 DSK_API int dsk_lsh_alive(const dsk_lsh *ix, const int32_t *d_docs, int64_t n, uint8_t *d_out, void *stream);
 DSK_API size_t dsk_lsh_compact_workspace_size(const dsk_lsh *ix);

@@ -32,10 +32,11 @@ def ev_time(fn, iters=3, warm=1):
     return e0.elapsed_time(e1) / iters
 
 
-def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, remove_leg=False):
+def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, remove_leg=False, query_jaccard_leg=False):
     """10M x 128 tokens, K=256 + LSH(0.8) insert + query (here n_docs on one GPU).  dedup_leg: also the self-join of
     the index (candidate_pairs, duplicate_clusters with and without min_jaccard=0.8) against the host flow it replaces.
-    remove_leg: also removal of the duplicates from the index and its compaction (c3_remove)."""
+    remove_leg: also removal of the duplicates from the index and its compaction (c3_remove).  query_jaccard_leg: also
+    queries verified on the device against the two-step flow they replace (c3_query_jaccard)."""
     perms = _make_permutations(k, 1)
     g = torch.Generator(device="cuda").manual_seed(3)
     tok = torch.randint(-2 ** 31, 2 ** 31 - 1, (n_docs, t), dtype=torch.int32, device="cuda", generator=g)
@@ -103,6 +104,8 @@ def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, 
     dedup = c3_dedup(lsh, src, dst, ref, hs) if dedup_leg else {}
     if remove_leg:
         dedup.update(c3_remove(lsh, sig, q))
+    if query_jaccard_leg:
+        dedup.update(c3_query_jaccard(lsh, sig, tok, perms))
     return {"config": "C3 (1 GPU)", "docs": n_docs, "tokens": t, "num_perm": k, "b": lsh.b, "r": lsh.r,
             "signature_ms": ms_sig, "signatures_per_s": n_docs / ms_sig * 1e3,
             "lsh_insert_ms": ms_ins, "lsh_insert_docs_per_s": n_docs / ms_ins * 1e3,
@@ -210,6 +213,80 @@ def c3_remove(lsh, sig, q, min_jaccard=0.8, rounds=3):
     return out
 
 
+def gpu_card():
+    """The card's name, power limit and top SM clock, read in the same process as the timings beside them."""
+    import subprocess
+    line = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                           "-i", str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+    name, watts, mhz = [s.strip() for s in line.split(",")]
+    return {"gpu": name, "power_limit_w": float(watts), "sm_clock_max_mhz": float(mhz)}
+
+
+def c3_query_jaccard(lsh, sig, tok, perms, n_query=100_000, min_jaccard=0.8, rounds=3):
+    """GpuLSH.query_jaccard / query_best for n_query fresh documents against the C3 index: half of them copies of indexed
+    documents with 10 % of the tokens resampled, half unrelated, their signatures built by the same kernel.  Beside them,
+    query() and the two-step flow they replace: query, the (query, document) pairs expanded with repeat_interleave,
+    codec.jaccard_pairs on cat([index rows, queries]) and the filter re-packed as CSR.  Each round times every call with
+    CUDA events (3 calls after 1 warm-up call), the calls alternating; the outputs are compared in the same run."""
+    n, k = len(lsh), lsh.h
+    t = tok.shape[1]
+    g = torch.Generator(device="cuda").manual_seed(11)
+    qtok = torch.randint(-2 ** 31, 2 ** 31 - 1, (n_query, t), dtype=torch.int32, device="cuda", generator=g)
+    h = n_query // 2
+    src = torch.randint(0, n, (h,), device="cuda", generator=g)
+    qtok[:h] = torch.where(torch.rand((h, t), device="cuda", generator=g) < 0.1, qtok[:h], tok[src])
+    qoff = torch.arange(0, (n_query + 1) * t, t, dtype=torch.int64, device="cuda")
+    qs = dsk.engine.bulk_signatures_device(qtok.view(-1), qoff, n_query * t, perms)
+    ar = torch.arange(n_query, device="cuda")
+
+    def two_step(thr):
+        p, x = lsh.query(qs, to_host=False)
+        rows = torch.repeat_interleave(ar, p[1:] - p[:-1])
+        jac = dsk.codec.jaccard_pairs(torch.cat([sig, qs]), rows + n, x.long())
+        keep = torch.from_numpy(jac >= thr).cuda()
+        cnt = torch.from_numpy(np.rint(jac * k).astype(np.int32)).cuda()
+        ptr = torch.zeros(n_query + 1, dtype=torch.int64, device="cuda")
+        ptr[1:] = torch.cumsum(torch.bincount(rows[keep], minlength=n_query), 0)
+        return ptr, x[keep], cnt[keep]
+
+    calls = {"query": lambda: lsh.query(qs, to_host=False),
+             "query_jaccard": lambda: lsh.query_jaccard(qs, to_host=False),
+             "query_jaccard_min_jaccard": lambda: lsh.query_jaccard(qs, min_jaccard, to_host=False),
+             "query_best_min_jaccard": lambda: lsh.query_best(qs, min_jaccard, to_host=False),
+             "two_step_min_jaccard": lambda: two_step(min_jaccard)}
+    times = {name: [] for name in calls}
+    for _ in range(rounds):
+        for name, fn in calls.items():
+            times[name].append(ev_time(fn))
+    # outputs: query_jaccard(min_jaccard) == the two-step flow (same sets, same eq); query_best == their per-query argmax
+    p1, x1, e1 = lsh.query_jaccard(qs, min_jaccard, to_host=False)
+    p2, x2, e2 = two_step(min_jaccard)
+    def keyed(p, x, e):
+        key = torch.repeat_interleave(ar, p[1:] - p[:-1]) * n + x.long()
+        order = torch.argsort(key)
+        return key[order], e[order]
+    k1, f1 = keyed(p1, x1, e1)
+    k2, f2 = keyed(p2, x2, e2)
+    same = bool(torch.equal(p1, p2)) and bool(torch.equal(k1, k2)) and bool(torch.equal(f1, f2))
+    rows = torch.repeat_interleave(ar, p2[1:] - p2[:-1])
+    score = e2.long() * (1 << 32) - x2.long()                # largest eq, then smallest document
+    top = torch.full((n_query,), -(1 << 62), dtype=torch.int64, device="cuda").scatter_reduce(0, rows, score, "amax")
+    w_eq = torch.where(top > -(1 << 62), (top + (1 << 32) - 1) >> 32, torch.full_like(top, -1))
+    w_idx = torch.where(w_eq >= 0, w_eq * (1 << 32) - top, torch.full_like(top, -1))
+    bi, bq = lsh.query_best(qs, min_jaccard, to_host=False)
+    best_same = bool(torch.equal(bi.long(), w_idx)) and bool(torch.equal(bq.long(), w_eq))
+    p0, _ = lsh.query(qs, to_host=False)
+    pa, _, _ = lsh.query_jaccard(qs, to_host=False)
+    out = {"qj_queries": n_query, "qj_min_jaccard": min_jaccard, "qj_candidates": int(p0[-1].item()),
+           "qj_candidates_unfiltered_equal_query": bool(torch.equal(p0, pa)), "qj_kept": int(p1[-1].item()),
+           "qj_queries_with_best": int((bi >= 0).sum().item()),
+           "qj_fused_equals_two_step": same, "qj_best_equals_two_step_argmax": best_same}
+    for name, ts in times.items():
+        out["qj_%s_ms" % name] = ts
+    out.update({"qj_" + key: v for key, v in gpu_card().items()})
+    return out
+
+
 def c4(n_vec, dim=4096, ss=128):
     gen = dsk.WeightedMinHashGenerator(dim, ss, 1)
     g = torch.Generator(device="cuda").manual_seed(4)
@@ -284,9 +361,13 @@ if __name__ == "__main__":
     ap.add_argument("--c3-remove", action="store_true",
                     help="after the dedup leg: GpuLSH.remove of the duplicates, the walks with removals present beside the "
                          "same calls without removals, and compact()")
+    ap.add_argument("--c3-query-jaccard", action="store_true",
+                    help="also time GpuLSH.query_jaccard / query_best for 100k fresh documents against the C3 index, beside "
+                         "query() and the two-step flow they replace, and compare their outputs")
     a = ap.parse_args()
     if a.c3_docs > 0:
-        print(json.dumps(c3(a.c3_docs, fused_leg=a.c3_fused, dedup_leg=a.c3_dedup, remove_leg=a.c3_remove)), flush=True)
+        print(json.dumps(c3(a.c3_docs, fused_leg=a.c3_fused, dedup_leg=a.c3_dedup, remove_leg=a.c3_remove,
+                            query_jaccard_leg=a.c3_query_jaccard)), flush=True)
     for fn, arg in ((c4, a.c4_vecs), (c5, a.c5_rows)):
         if arg > 0:
             print(json.dumps(fn(arg)), flush=True)
