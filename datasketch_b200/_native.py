@@ -64,6 +64,10 @@ SIGNATURES = {
     "dsk_lsh_query_jaccard_count": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
     "dsk_lsh_query_jaccard_fill": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dsk_lsh_query_best": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    "dsk_lsh_unique_workspace_size": (ctypes.c_size_t, [c_void_p, c_int64]),
+    "dsk_lsh_unique_count": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "dsk_lsh_unique_commit": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_size_t, c_void_p, c_void_p,
+                                      c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_int64), c_void_p]),
     "dsk_lsh_remove": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "dsk_lsh_alive": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "dsk_lsh_compact_workspace_size": (ctypes.c_size_t, [c_void_p]),

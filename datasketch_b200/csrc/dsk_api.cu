@@ -162,6 +162,15 @@ struct dsk_lsh {
     uint32_t *removed = nullptr;   // removal bitmap, (cap_docs + 31) / 32 words: allocated by the first dsk_lsh_remove
     bool has_removals = false;     // a dsk_lsh_remove since the last compaction: the walks run their removal-aware kernels
     const uint32_t *walk_bitmap() const { return has_removals ? removed : nullptr; }
+    uint64_t changes = 0;          // bumped by every call that changes the index (insert, removal, compaction)
+    mutable struct {               // the last dsk_lsh_unique_count, which dsk_lsh_unique_commit must follow
+        bool armed;
+        const uint32_t *sig;
+        const void *ws;
+        int64_t n;
+        int min_count;
+        uint64_t changes;
+    } unique{};
 };
 
 extern "C" {
@@ -723,6 +732,7 @@ int dsk_lsh_insert(dsk_lsh *ix, const uint32_t *d_sig, int64_t n, void *stream) 
     DevGuard guard(ix->device);
     DSK_CUDA(launch_lsh_insert(ix->dev, d_sig, ix->n_docs, n, dev->sm_count, (cudaStream_t)stream));
     ix->n_docs += n;
+    ++ix->changes;
     return DSK_OK;
 }
 
@@ -784,6 +794,7 @@ int dsk_lsh_insert_tokens(dsk_lsh *ix, const dsk_perm *perm, const void *d_token
     if (!fused)   // rows are in place already: the insert kernel's copy of them is a self-copy
         DSK_CUDA(launch_lsh_insert(ix->dev, rows, ix->n_docs, n_docs, dev->sm_count, (cudaStream_t)stream));
     ix->n_docs += n_docs;
+    ++ix->changes;
     return DSK_OK;
 }
 
@@ -970,6 +981,7 @@ int dsk_lsh_remove(dsk_lsh *ix, const int32_t *d_docs, int64_t n, int64_t *d_sta
         ix->removed = bits;
     }
     ix->has_removals = true;
+    ++ix->changes;
     DSK_CUDA(launch_lsh_remove(ix->removed, d_docs, n, ix->n_docs, d_status, dev->sm_count, (cudaStream_t)stream));
     return DSK_OK;
 }
@@ -1023,6 +1035,90 @@ int dsk_lsh_compact(dsk_lsh *ix, int32_t *d_remap, void *d_ws, size_t ws_bytes, 
     DSK_CUDA(cudaMemsetAsync(ix->removed, 0, (size_t)(n + 31) / 32 * sizeof(uint32_t), s));
     ix->has_removals = false;
     ix->n_docs = m;
+    ++ix->changes;
+    return DSK_OK;
+}
+
+// ---- insert_unique: count (batch table, stage A, earlier partners) -> dsk_exclusive_scan -> commit ----------------------
+size_t dsk_lsh_unique_workspace_size(const dsk_lsh *ix, int64_t n) {
+    return ix && n > 0 ? lsh_unique_workspace_bytes(ix->dev, n) : 0;
+}
+
+// handle, n >= 0, min_count in [0, num_perm], and for n > 0 the rows, a 16-byte aligned workspace of the size
+// dsk_lsh_unique_workspace_size gives and every buffer (bufs)
+static int check_unique(const char *who, const dsk_lsh *ix, const uint32_t *d_sig, int64_t n, int min_count, const void *d_ws,
+                        size_t ws_bytes, bool bufs) {
+    int rc = check_self_join(who, ix, min_count);
+    if (rc) return rc;
+    if (n < 0) {
+        set_error("%s: n must be >= 0 (got %lld)", who, (long long)n);
+        return DSK_ERR_INVALID;
+    }
+    if (n == 0) return DSK_OK;
+    if (!d_sig || !d_ws || !bufs) {
+        set_error("%s: null buffer", who);
+        return DSK_ERR_INVALID;
+    }
+    const size_t need = lsh_unique_workspace_bytes(ix->dev, n);
+    if (((uintptr_t)d_ws & 15) != 0 || ws_bytes < need) {
+        set_error("%s: the workspace must be 16-byte aligned and hold dsk_lsh_unique_workspace_size() = %zu bytes (got %zu)",
+                  who, need, ws_bytes);
+        return DSK_ERR_INVALID;
+    }
+    return DSK_OK;
+}
+
+int dsk_lsh_unique_count(const dsk_lsh *ix, const uint32_t *d_sig, int64_t n, int min_count, void *d_ws, size_t ws_bytes,
+                         int64_t *d_counts, void *stream) {
+    int rc = check_unique("dsk_lsh_unique_count", ix, d_sig, n, min_count, d_ws, ws_bytes, d_counts != nullptr);
+    if (rc) return rc;
+    ix->unique.armed = false;
+    if (n == 0) return DSK_OK;
+    DevInfo *dev;
+    rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    DSK_CUDA(lsh_unique_count(ix->dev, ix->n_docs, d_sig, n, min_count, d_ws, d_counts, ix->walk_bitmap(), dev->sm_count,
+                              (cudaStream_t)stream));
+    ix->unique = {true, d_sig, d_ws, n, min_count, ix->changes};
+    return DSK_OK;
+}
+
+int dsk_lsh_unique_commit(dsk_lsh *ix, const uint32_t *d_sig, int64_t n, int min_count, void *d_ws, size_t ws_bytes,
+                          const int64_t *d_ptr, int32_t *d_pidx, int32_t *d_peq, uint8_t *d_kept, int32_t *d_match,
+                          int32_t *d_eq, int64_t *h_inserted, void *stream) {
+    int rc = check_unique("dsk_lsh_unique_commit", ix, d_sig, n, min_count, d_ws, ws_bytes,
+                          d_ptr && d_pidx && d_peq && d_kept && d_match && d_eq && h_inserted);
+    if (rc) return rc;
+    if (n == 0) {
+        if (h_inserted) *h_inserted = 0;
+        return DSK_OK;
+    }
+    const auto &u = ix->unique;
+    if (!u.armed || u.sig != d_sig || u.ws != d_ws || u.n != n || u.min_count != min_count || u.changes != ix->changes) {
+        set_error("dsk_lsh_unique_commit: must follow dsk_lsh_unique_count of the same d_sig, n, min_count and d_ws, with no "
+                  "change of the index in between");
+        return DSK_ERR_INVALID;
+    }
+    ix->unique.armed = false;
+    DevInfo *dev;
+    rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    const cudaStream_t s = (cudaStream_t)stream;
+    int64_t m = 0;
+    DSK_CUDA(lsh_unique_resolve(ix->dev, ix->n_docs, d_sig, n, min_count, d_ws, d_ptr, d_pidx, d_peq, d_kept, d_match, d_eq,
+                                &m, dev->sm_count, s));
+    *h_inserted = 0;
+    if (ix->n_docs + m > ix->dev.cap_docs) {
+        set_error("dsk_lsh_unique_commit: capacity exceeded (%lld + %lld kept > %lld); the index is unchanged",
+                  (long long)ix->n_docs, (long long)m, (long long)ix->dev.cap_docs);
+        return DSK_ERR_INVALID;
+    }
+    DSK_CUDA(lsh_unique_insert(ix->dev, ix->n_docs, d_sig, n, m, d_ws, dev->sm_count, s));
+    ix->n_docs += m;
+    ++ix->changes;
+    *h_inserted = m;
     return DSK_OK;
 }
 

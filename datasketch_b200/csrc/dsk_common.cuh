@@ -150,6 +150,16 @@ size_t lsh_compact_workspace_bytes(int64_t n_docs, int k);
 cudaError_t launch_lsh_identity(int32_t *remap, int64_t n, int sm_count, cudaStream_t s);   // remap[i] = i
 cudaError_t lsh_compact(const LshDev &ix, const uint32_t *removed, int64_t n_docs, int32_t *remap, void *ws, int64_t *m,
                         int sm_count, cudaStream_t s);
+// insert_unique (the streaming dedup loop over a batch of n rows): workspace bytes; the batch table, stage A and the counts
+// of the earlier partners; the fill, resolution and matches (*m = kept rows, one synchronisation); the insert of the kept
+size_t lsh_unique_workspace_bytes(const LshDev &ix, int64_t n);
+cudaError_t lsh_unique_count(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
+                             int64_t *counts, const uint32_t *removed, int sm_count, cudaStream_t s);
+cudaError_t lsh_unique_resolve(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
+                               const int64_t *ptr, int32_t *pidx, int32_t *peq, uint8_t *kept, int32_t *match, int32_t *eq,
+                               int64_t *m, int sm_count, cudaStream_t s);
+cudaError_t lsh_unique_insert(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int64_t m, void *ws,
+                              int sm_count, cudaStream_t s);
 
 cudaError_t launch_jaccard_pairs(const uint32_t *sig, int64_t n_rows, int k, const int64_t *ia, const int64_t *ib,
                                  int64_t m, int32_t *out, int sm_count, cudaStream_t s);

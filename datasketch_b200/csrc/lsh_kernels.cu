@@ -814,3 +814,235 @@ cudaError_t lsh_compact(const LshDev &ix, const uint32_t *removed, int64_t n_doc
 }
 
 }  // namespace dsk
+
+// ---- insert_unique: the streaming dedup loop over a batch --------------------------------------------------------------
+// for each row j of the batch, in order: keep j (insert it) iff no remaining document of the index and no row j' < j of the
+// batch that was kept is a candidate of j with eq >= min_count.  Three relations decide it:
+//   stage A       the self-join's QUERY_BEST walk of every row against the index (removal-aware): a row with a kept
+//                 candidate there is DROPPED whatever the batch holds, and its (idx, eq) is the index's side of its match;
+//   batch pairs   a second LshDev over the batch rows themselves (a table in the caller's workspace, filled by
+//                 lsh_insert_kernel, which skips its row copy because the rows already are the table's rows), whose
+//                 PAIRS_COUNT / PAIRS_FILL walk lists every row's earlier partners d < j with eq >= min_count as CSR;
+//   resolution    statuses UNDECIDED -> KEPT / DROPPED: a row with a KEPT earlier partner is DROPPED, a row whose earlier
+//                 partners are all DROPPED (or that has none) is KEPT, any other row waits.
+// A status is written once, from UNDECIDED to final, and a decision is taken from final statuses only, so by induction in
+// row order every decision is the loop's, whichever order the threads visit the rows in and whichever of the other threads'
+// writes of the same round they see: statuses are read and written with relaxed atomics.  The smallest undecided row can
+// always decide, so every round decides at least one row; a drift chain (row j's only partner is j - 1) of length L takes
+// about L rounds.  The rounds run as kUniqueSweeps grid-wide sweeps (one launch each, no host synchronisation), the last
+// of which lists the rows still undecided; one CTA then loops over that list, round after round, separated by
+// __syncthreads, until it is empty.  No CTA ever waits for another.
+namespace dsk {
+
+enum : int32_t { kUndecided = 0, kKept = 1, kDropped = 2 };
+constexpr int kUniqueSweeps = 3;           // grid-wide rounds before the remainder goes to one CTA
+constexpr int kResolveThreads = 1024;      // the CTA that finishes the rounds
+
+// Decides row j from the statuses of its earlier partners pidx[ptr[j] .. ptr[j + 1]); false: j stays undecided.
+__device__ __forceinline__ bool unique_decide(const int64_t *ptr, const int32_t *pidx, int32_t *st, int64_t j) {
+    bool open = false;
+    for (int64_t p = ptr[j]; p < ptr[j + 1]; ++p) {
+        const int32_t s = ld_relaxed(st + pidx[p]);
+        if (s == kKept) {
+            st_relaxed(st + j, kDropped);
+            return true;
+        }
+        open = open || s == kUndecided;
+    }
+    if (open) return false;
+    st_relaxed(st + j, kKept);
+    return true;
+}
+
+// st[j] = DROPPED for a row with a kept candidate in the index (stage A), else UNDECIDED
+__global__ void __launch_bounds__(256) unique_init_kernel(const int32_t *__restrict__ aidx, int64_t n, int32_t *st) {
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x)
+        st[j] = aidx[j] >= 0 ? kDropped : kUndecided;
+}
+
+// one grid-wide round over every undecided row; list != nullptr: appends the rows that stay undecided (in any order)
+__global__ void __launch_bounds__(256) unique_sweep_kernel(const int64_t *__restrict__ ptr, const int32_t *__restrict__ pidx,
+                                                           int32_t *st, int64_t n, int32_t *list, unsigned *list_n) {
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+        if (ld_relaxed(st + j) != kUndecided) continue;
+        if (!unique_decide(ptr, pidx, st, j) && list) list[atomicAdd(list_n, 1u)] = (int32_t)j;
+    }
+}
+
+// ONE CTA: rounds over the listed rows until every row is decided; each round lists its still undecided rows in the other
+// buffer.  Every round decides at least the smallest listed row, so the loop ends.
+__global__ void __launch_bounds__(kResolveThreads) unique_resolve_kernel(const int64_t *__restrict__ ptr,
+                                                                         const int32_t *__restrict__ pidx, int32_t *st,
+                                                                         int32_t *list, int32_t *spare,
+                                                                         const unsigned *list_n) {
+    __shared__ unsigned s_left;
+    unsigned left = *list_n;
+    int32_t *cur = list, *nxt = spare;
+    while (left > 0) {
+        __syncthreads();   // every thread has read s_left before it is reset
+        if (threadIdx.x == 0) s_left = 0;
+        __syncthreads();
+        for (unsigned i = threadIdx.x; i < left; i += blockDim.x) {
+            const int32_t j = cur[i];
+            if (!unique_decide(ptr, pidx, st, j)) nxt[atomicAdd(&s_left, 1u)] = j;
+        }
+        __syncthreads();
+        left = s_left;
+        int32_t *t = cur;
+        cur = nxt;
+        nxt = t;
+    }
+}
+
+// flags[j] = 1 for a kept row (the exclusive scan of the flags numbers the kept rows), kept[j] the caller's copy
+__global__ void __launch_bounds__(256) unique_flags_kernel(const int32_t *__restrict__ st, int64_t n,
+                                                           int64_t *__restrict__ flags, uint8_t *__restrict__ kept) {
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+        const bool k = st[j] == kKept;
+        flags[j] = k;
+        kept[j] = k;
+    }
+}
+
+// A kept row: match / eq = -1, new2old[rank] = j.  A dropped row: the best of stage A's (idx, eq) and its KEPT earlier
+// partners (n0 + rank, eq) -- the largest eq, then the smallest document number, so an indexed document (< n0) wins a tie.
+__global__ void __launch_bounds__(256) unique_match_kernel(const int32_t *__restrict__ st, const int64_t *__restrict__ ptr,
+                                                           const int32_t *__restrict__ pidx, const int32_t *__restrict__ peq,
+                                                           const int32_t *__restrict__ aidx, const int32_t *__restrict__ aeq,
+                                                           const int64_t *__restrict__ rank, int64_t n0, int64_t n,
+                                                           int32_t *__restrict__ match, int32_t *__restrict__ eq,
+                                                           int32_t *__restrict__ new2old) {
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+        if (st[j] == kKept) {
+            match[j] = -1;
+            eq[j] = -1;
+            new2old[rank[j]] = (int32_t)j;
+            continue;
+        }
+        int32_t bd = aidx[j], be = aeq[j];
+        for (int64_t p = ptr[j]; p < ptr[j + 1]; ++p) {
+            const int32_t d = pidx[p];
+            if (st[d] != kKept) continue;
+            const int32_t c = (int32_t)(n0 + rank[d]), e = peq[p];
+            if (e > be || (e == be && c < bd)) { bd = c; be = e; }
+        }
+        match[j] = bd;
+        eq[j] = be;
+    }
+}
+
+// workspace of a batch of n rows: the batch table's slots [b][cap_slots][2] u64 and next [n][b] i32 | stage A's idx, eq
+// i32[n] | statuses i32[n] | kept flags i64[n] | ranks i64[n + 1] | scan scratch i64[n / 1024 + 2] | two lists i32[n] |
+// new -> old i32[n] | the list counter.  Each part 256-byte aligned.
+static int64_t unique_cap_slots(int64_t n) {
+    int64_t c = 2;
+    while (c < 2 * n) c <<= 1;
+    return c;
+}
+
+struct UniqueWs {
+    LshDev bt;   // the batch table (sig = the batch rows)
+    int32_t *aidx, *aeq, *st, *list, *spare, *new2old;
+    int64_t *flags, *rank, *scratch;
+    unsigned *list_n;
+};
+
+static UniqueWs unique_ws(void *ws, const LshDev &ix, const uint32_t *sig, int64_t n, size_t *bytes) {
+    UniqueWs w{};
+    char *p = static_cast<char *>(ws);
+    size_t off = 0;
+    auto take = [&](size_t sz) { char *q = p ? p + off : nullptr; off += align256(sz); return q; };
+    w.bt.cap_slots = unique_cap_slots(n);
+    w.bt.slots = reinterpret_cast<uint64_t *>(take((size_t)ix.b * w.bt.cap_slots * 16));
+    w.bt.next = reinterpret_cast<int32_t *>(take((size_t)n * ix.b * 4));
+    w.bt.sig = const_cast<uint32_t *>(sig);   // read only: lsh_insert_kernel does not copy rows onto themselves
+    w.bt.cap_docs = n;
+    w.bt.k = ix.k;
+    w.bt.b = ix.b;
+    w.bt.r = ix.r;
+    w.aidx = reinterpret_cast<int32_t *>(take((size_t)n * 4));
+    w.aeq = reinterpret_cast<int32_t *>(take((size_t)n * 4));
+    w.st = reinterpret_cast<int32_t *>(take((size_t)n * 4));
+    w.flags = reinterpret_cast<int64_t *>(take((size_t)n * 8));
+    w.rank = reinterpret_cast<int64_t *>(take((size_t)(n + 1) * 8));
+    w.scratch = reinterpret_cast<int64_t *>(take((size_t)(n / 1024 + 2) * 8));
+    w.list = reinterpret_cast<int32_t *>(take((size_t)n * 4));
+    w.spare = reinterpret_cast<int32_t *>(take((size_t)n * 4));
+    w.new2old = reinterpret_cast<int32_t *>(take((size_t)n * 4));
+    w.list_n = reinterpret_cast<unsigned *>(take(16));
+    if (bytes) *bytes = off;
+    return w;
+}
+
+size_t lsh_unique_workspace_bytes(const LshDev &ix, int64_t n) {
+    if (n <= 0) return 0;
+    size_t bytes = 0;
+    unique_ws(nullptr, ix, nullptr, n, &bytes);
+    return bytes;
+}
+
+static unsigned unique_grid(int64_t work, int sm_count) {
+    int64_t g = (work + 255) / 256;
+    if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
+    return (unsigned)(g < 1 ? 1 : g);
+}
+
+// Builds the batch table over sig (n rows), runs stage A against the first n_docs documents of ix, and writes counts[j] =
+// the number of row j's earlier partners in the batch.  No synchronisation.
+cudaError_t lsh_unique_count(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
+                             int64_t *counts, const uint32_t *removed, int sm_count, cudaStream_t s) {
+    const UniqueWs w = unique_ws(ws, ix, sig, n, nullptr);
+    cudaError_t e = cudaMemsetAsync(w.bt.slots, 0xFF, (size_t)ix.b * w.bt.cap_slots * 16, s);   // empty key, head -1
+    if (e == cudaSuccess) e = launch_lsh_insert(w.bt, sig, 0, n, sm_count, s);
+    if (e == cudaSuccess)
+        e = launch_lsh_query_pairs(ix, sig, n, n_docs, min_count, nullptr, nullptr, w.aidx, w.aeq, removed, sm_count, s);
+    if (e == cudaSuccess) e = launch_lsh_pairs(w.bt, n, min_count, counts, nullptr, nullptr, nullptr, nullptr, sm_count, s);
+    return e;
+}
+
+// After lsh_unique_count and the scan of its counts into ptr: fills the batch pairs (pidx / peq), resolves the statuses,
+// writes kept / match / eq and new -> old, and returns *m = the number of kept rows.  Synchronises s once, to read m.
+cudaError_t lsh_unique_resolve(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
+                               const int64_t *ptr, int32_t *pidx, int32_t *peq, uint8_t *kept, int32_t *match, int32_t *eq,
+                               int64_t *m, int sm_count, cudaStream_t s) {
+    const UniqueWs w = unique_ws(ws, ix, sig, n, nullptr);
+    const unsigned grid = unique_grid(n, sm_count);
+    cudaError_t e = launch_lsh_pairs(w.bt, n, min_count, nullptr, ptr, pidx, peq, nullptr, sm_count, s);
+    if (e != cudaSuccess) return e;
+    DSK_LAUNCH(unique_init_kernel, grid, 256, 0, s, w.aidx, n, w.st);
+    e = cudaMemsetAsync(w.list_n, 0, sizeof(unsigned), s);
+    if (e != cudaSuccess) return e;
+    for (int round = 0; round < kUniqueSweeps; ++round) {
+        const bool last = round == kUniqueSweeps - 1;
+        DSK_LAUNCH(unique_sweep_kernel, grid, 256, 0, s, ptr, (const int32_t *)pidx, w.st, n, last ? w.list : nullptr,
+                   w.list_n);
+    }
+    DSK_LAUNCH(unique_resolve_kernel, 1, kResolveThreads, 0, s, ptr, (const int32_t *)pidx, w.st, w.list, w.spare,
+               (const unsigned *)w.list_n);
+    DSK_LAUNCH(unique_flags_kernel, grid, 256, 0, s, (const int32_t *)w.st, n, w.flags, kept);
+    e = launch_exclusive_scan(w.flags, n, w.rank, w.scratch, s);
+    if (e != cudaSuccess) return e;
+    DSK_LAUNCH(unique_match_kernel, grid, 256, 0, s, (const int32_t *)w.st, ptr, (const int32_t *)pidx,
+               (const int32_t *)peq, (const int32_t *)w.aidx, (const int32_t *)w.aeq, (const int64_t *)w.rank, n_docs, n,
+               match, eq, w.new2old);
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(m, w.rank + n, sizeof(int64_t), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    return e;
+}
+
+// After lsh_unique_resolve: the m kept rows gathered into the index's storage behind its n_docs documents, then inserted
+// there as documents n_docs .. n_docs + m - 1 (lsh_insert_kernel's copy is a self-copy).  The caller checked the capacity.
+cudaError_t lsh_unique_insert(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int64_t m, void *ws,
+                              int sm_count, cudaStream_t s) {
+    if (m <= 0) return cudaSuccess;
+    const UniqueWs w = unique_ws(ws, ix, sig, n, nullptr);
+    uint32_t *dst = ix.sig + n_docs * ix.k;
+    DSK_LAUNCH(compact_gather_kernel, unique_grid(m * 32, sm_count), 256, 0, s, sig, ix.k, (const int32_t *)w.new2old,
+               (int64_t)0, m, dst);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = launch_lsh_insert(ix, dst, n_docs, m, sm_count, s);
+    return e;
+}
+
+}  // namespace dsk

@@ -667,6 +667,70 @@ class GpuLSH:
             return idx.cpu().numpy(), eq.cpu().numpy()
         return idx, eq
 
+    # -- streaming de-duplication: insert the rows that have no near-duplicate yet ---------------------------------------
+    def insert_unique(self, sig, min_jaccard: Optional[float] = None, keys: Optional[Iterable[Hashable]] = None,
+                      to_host: bool = True):
+        """Insert the rows of ``sig`` that have no near-duplicate yet: ``(kept bool[B], match int32[B], eq int32[B])``.
+
+        The result is, row for row, that of the streaming de-duplication loop over the batch in order::
+
+            for j, m in enumerate(sig):
+                if not [d for d in lsh.query(m) if m.jaccard(doc[d]) >= min_jaccard]:
+                    lsh.insert(key[j], m)
+
+        Row j is kept iff no remaining (not removed) document of the index and no row of this batch kept before j is a
+        candidate of row j with ``MinHash.jaccard >= min_jaccard`` (``min_jaccard=None``: any candidate drops the row).
+        The kept rows become documents ``len(self), len(self) + 1, ...`` in batch order, and ``keys`` (one per row, when
+        given) is appended for the kept rows only.  For a dropped row, ``match`` / ``eq`` give the candidate of the loop's
+        query with the largest ``eq`` (the number of agreeing positions; ``eq / num_perm`` is ``MinHash.jaccard``), the
+        smallest document number among equal ones, with the numbers the documents have after the call: an indexed
+        document wins a tie against a row of the batch.  Both are -1 for a kept row.
+
+        This differs from ``duplicate_clusters``, which keeps one document per connected component: in a drift chain
+        a ~ b ~ c where a and c do not match, the loop keeps a and c (b is dropped, so nothing kept matches c), while
+        the component {a, b, c} keeps only a.
+
+        If the kept rows do not fit the capacity, raises ``ValueError`` and changes nothing: the index, ``len()`` and
+        ``keys`` are as before.  Runs on the device and waits for it twice: for the size of the batch's pair list and
+        for the number of kept rows."""
+        import torch
+        mc = _jaccard_min_count(min_jaccard, self.h)
+        d_sig = self._dev_sig(sig)
+        n = d_sig.shape[0]
+        if keys is not None:
+            keys = list(keys)
+            if len(keys) != n:
+                raise ValueError("keys must hold one key per row of sig (%d), got %d" % (n, len(keys)))
+        lib = nv.load()
+        dev = d_sig.device
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream().cuda_stream
+            ws_bytes = int(lib.dsk_lsh_unique_workspace_size(self._h, n))
+            ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
+            counts = torch.empty((max(n, 1),), dtype=torch.int64, device=dev)
+            ptr = torch.empty((n + 1,), dtype=torch.int64, device=dev)
+            scratch = torch.empty((n // 1024 + 2,), dtype=torch.int64, device=dev)
+            nv.check(lib.dsk_lsh_unique_count(self._h, d_sig.data_ptr(), n, mc, ws.data_ptr(), ws_bytes,
+                                              counts.data_ptr(), st))
+            nv.check(lib.dsk_exclusive_scan(counts.data_ptr(), n, ptr.data_ptr(), scratch.data_ptr(), st))
+            total = int(ptr[n].item())
+            pidx = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
+            peq = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
+            kept = torch.empty((max(n, 1),), dtype=torch.uint8, device=dev)
+            match = torch.empty((max(n, 1),), dtype=torch.int32, device=dev)
+            eq = torch.empty((max(n, 1),), dtype=torch.int32, device=dev)
+            inserted = ctypes.c_int64(0)
+            nv.check(lib.dsk_lsh_unique_commit(self._h, d_sig.data_ptr(), n, mc, ws.data_ptr(), ws_bytes, ptr.data_ptr(),
+                                               pidx.data_ptr(), peq.data_ptr(), kept.data_ptr(), match.data_ptr(),
+                                               eq.data_ptr(), ctypes.byref(inserted), st))
+            kept, match, eq = kept[:n].bool(), match[:n], eq[:n]
+        if keys is not None:
+            mask = kept.cpu().numpy()
+            self.keys.extend(k for k, keep in zip(keys, mask) if keep)
+        if to_host:
+            return kept.cpu().numpy(), match.cpu().numpy(), eq.cpu().numpy()
+        return kept, match, eq
+
     # -- self-join: near-duplicate pairs and clusters of the indexed documents ------------------------------------------
     def candidate_pairs(self, min_jaccard: Optional[float] = None, to_host: bool = True):
         """Every candidate pair among the ``n = len(self)`` indexed documents, once, as CSR arrays

@@ -284,6 +284,38 @@ DSK_API int dsk_lsh_query_jaccard_fill(const dsk_lsh *ix, const uint32_t *d_qsig
                                        const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq, void *stream);
 DSK_API int dsk_lsh_query_best(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, int32_t *d_idx,
                                int32_t *d_eq, void *stream);
+/* Streaming de-duplication of a batch (the loop `for m in batch: if not [d for d in lsh.query(m) if m.jaccard(doc[d]) >= t]:
+ * lsh.insert(key, m)`, lsh.py:326-347 / :370-432, minhash.py:299-324), on the device.  Row j of d_sig ([n, num_perm] u32)
+ * is KEPT iff no remaining (not removed) document of the index and no row j' < j of the batch that was kept is a candidate
+ * of row j with eq >= min_count (min_count in [0, num_perm]; 0: any candidate drops the row).  The kept rows are inserted in
+ * batch order as documents n_docs, n_docs + 1, ...; afterwards the index equals one into which the loop inserted them.
+ *   dsk_lsh_unique_workspace_size  bytes of d_ws (16-byte aligned) for n rows: the batch's own bucket table, cap_slots =
+ *                        the smallest power of two >= 2n (at least 2), i.e. 16 * b * cap_slots + 4 * b * n bytes, about
+ *                        32 * b * n + 4 * b * n; plus about 40 * n bytes for stage A's idx / eq, the statuses, the kept flags and
+ *                        their scan, two row lists and new -> old; each part rounded up to 256 bytes.  0 for n <= 0.
+ *   dsk_lsh_unique_count builds the batch table over d_sig, walks every row against the index (the best kept candidate
+ *                        there, as dsk_lsh_query_best) and writes d_counts[j] = the number of rows d < j of the batch that
+ *                        are candidates of row j with eq >= min_count.  Asynchronous, no synchronisation.
+ *   dsk_lsh_unique_commit after dsk_exclusive_scan of the counts into d_ptr (n + 1 entries): writes the batch pairs into
+ *                        d_pidx / d_peq (d_ptr[n] entries each), resolves the loop's decisions, then writes d_kept[j]
+ *                        (1 / 0) and, for a dropped row, d_match[j] / d_eq[j] = the candidate of the loop's query with the
+ *                        largest eq, the smallest document number among equal ones (numbers after the call: indexed
+ *                        documents win ties against batch rows); -1 / -1 for a kept row.  It SYNCHRONISES the stream once,
+ *                        to read the number m of kept rows; if n_docs + m > capacity_docs it returns DSK_ERR_INVALID with
+ *                        the index unchanged (the outputs are written), else it inserts the kept rows and sets
+ *                        *h_inserted = m (host memory).
+ * The commit must follow the count with the same d_sig, n, min_count and d_ws (the workspace carries the batch table and
+ * stage A's results between them) and with no change of the index in between; anything else is DSK_ERR_INVALID.  Both
+ * check the handle, n >= 0, min_count, the workspace and the buffers; n == 0 with null buffers is a valid no-op.  Cost: the
+ * batch walk is quadratic in the size of each within-batch bucket (as dsk_lsh_pairs_* with min_count > 0); the resolution
+ * takes about as many rounds as the longest chain of rows whose decisions wait for each other (a drift chain of L rows:
+ * ~L rounds), run by one CTA after three grid-wide sweeps, without host synchronisation. */
+DSK_API size_t dsk_lsh_unique_workspace_size(const dsk_lsh *ix, int64_t n);
+DSK_API int dsk_lsh_unique_count(const dsk_lsh *ix, const uint32_t *d_sig, int64_t n, int min_count, void *d_ws,
+                                 size_t ws_bytes, int64_t *d_counts, void *stream);
+DSK_API int dsk_lsh_unique_commit(dsk_lsh *ix, const uint32_t *d_sig, int64_t n, int min_count, void *d_ws, size_t ws_bytes,
+                                  const int64_t *d_ptr, int32_t *d_pidx, int32_t *d_peq, uint8_t *d_kept, int32_t *d_match,
+                                  int32_t *d_eq, int64_t *h_inserted, void *stream);
 DSK_API int dsk_lsh_remove(dsk_lsh *ix, const int32_t *d_docs, int64_t n, int64_t *d_status, void *stream);
 DSK_API int dsk_lsh_alive(const dsk_lsh *ix, const int32_t *d_docs, int64_t n, uint8_t *d_out, void *stream);
 DSK_API size_t dsk_lsh_compact_workspace_size(const dsk_lsh *ix);

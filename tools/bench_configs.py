@@ -32,11 +32,14 @@ def ev_time(fn, iters=3, warm=1):
     return e0.elapsed_time(e1) / iters
 
 
-def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, remove_leg=False, query_jaccard_leg=False):
+def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, remove_leg=False, query_jaccard_leg=False,
+       insert_unique_leg=False, n_unique=100_000):
     """10M x 128 tokens, K=256 + LSH(0.8) insert + query (here n_docs on one GPU).  dedup_leg: also the self-join of
     the index (candidate_pairs, duplicate_clusters with and without min_jaccard=0.8) against the host flow it replaces.
     remove_leg: also removal of the duplicates from the index and its compaction (c3_remove).  query_jaccard_leg: also
-    queries verified on the device against the two-step flow they replace (c3_query_jaccard)."""
+    queries verified on the device against the two-step flow they replace (c3_query_jaccard).  insert_unique_leg: also
+    GpuLSH.insert_unique of a batch of n_unique fresh documents against the flow it replaces (c3_insert_unique); the index
+    then has room for them (its bucket tables are the same size)."""
     perms = _make_permutations(k, 1)
     g = torch.Generator(device="cuda").manual_seed(3)
     tok = torch.randint(-2 ** 31, 2 ** 31 - 1, (n_docs, t), dtype=torch.int32, device="cuda", generator=g)
@@ -54,7 +57,7 @@ def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, 
     warm.insert(sig[:4096])                      # first launch of the kernels (module load, attribute set) is not timed
     warm.query(sig[:64], to_host=False)
     del warm
-    lsh = dsk.GpuLSH(threshold=0.8, num_perm=k, capacity=n_docs)
+    lsh = dsk.GpuLSH(threshold=0.8, num_perm=k, capacity=n_docs + (n_unique if insert_unique_leg else 0))
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
@@ -106,6 +109,8 @@ def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, 
         dedup.update(c3_remove(lsh, sig, q))
     if query_jaccard_leg:
         dedup.update(c3_query_jaccard(lsh, sig, tok, perms))
+    if insert_unique_leg:
+        dedup.update(c3_insert_unique(lsh, tok, perms, n_unique))
     return {"config": "C3 (1 GPU)", "docs": n_docs, "tokens": t, "num_perm": k, "b": lsh.b, "r": lsh.r,
             "signature_ms": ms_sig, "signatures_per_s": n_docs / ms_sig * 1e3,
             "lsh_insert_ms": ms_ins, "lsh_insert_docs_per_s": n_docs / ms_ins * 1e3,
@@ -287,6 +292,111 @@ def c3_query_jaccard(lsh, sig, tok, perms, n_query=100_000, min_jaccard=0.8, rou
     return out
 
 
+def c3_unique_batch(tok, nb, g, chain=5, drift=0.05):
+    """nb fresh token rows for a dedup batch against the documents `tok`: 40 % copies of indexed documents with 10 % of
+    the tokens resampled, 20 % unrelated, 20 % drift chains of `chain` rows (each row its predecessor with `drift` of the
+    tokens resampled) and 20 % exact copies of earlier rows of the batch, in that order."""
+    n, t = tok.shape
+    out = torch.randint(-2 ** 31, 2 ** 31 - 1, (nb, t), dtype=torch.int32, device="cuda", generator=g)
+    a, b = int(nb * 0.4), int(nb * 0.2)
+    c = int(nb * 0.2) // chain * chain
+    src = torch.randint(0, n, (a,), device="cuda", generator=g)
+    out[:a] = torch.where(torch.rand((a, t), device="cuda", generator=g) < 0.1, out[:a], tok[src])
+    s0 = a + b                                                  # chain i holds rows s0 + i * chain + 0 .. chain - 1
+    for step in range(1, chain):
+        cur = out[s0 + step:s0 + c:chain]
+        prev = out[s0 + step - 1:s0 + c:chain]
+        out[s0 + step:s0 + c:chain] = torch.where(torch.rand(cur.shape, device="cuda", generator=g) < drift, cur, prev)
+    csrc = torch.randint(0, a + b + c, (nb - a - b - c,), device="cuda", generator=g)
+    out[a + b + c:] = out[csrc]
+    return out
+
+
+def two_step_unique(lsh, bsig, min_jaccard):
+    """The flow GpuLSH.insert_unique replaces: query_best of the batch against the index, a temporary GpuLSH over the
+    batch and its candidate_pairs(min_jaccard), the greedy loop over those pairs on the host, then insert of the kept
+    rows.  Returns (kept, match, eq) as insert_unique does."""
+    n0, nb = len(lsh), bsig.shape[0]
+    bi, bq = lsh.query_best(bsig, min_jaccard)
+    tmp = dsk.GpuLSH(num_perm=lsh.h, params=(lsh.b, lsh.r), capacity=max(nb, 1))
+    tmp.insert(bsig)
+    ptr, idx, eq = tmp.candidate_pairs(min_jaccard)
+    del tmp
+    ptr, idx, eq = ptr.tolist(), idx.tolist(), eq.tolist()
+    kept = np.zeros(nb, dtype=bool)
+    rank = np.full(nb, -1, dtype=np.int64)
+    match, best = bi.astype(np.int64), bq.astype(np.int64)
+    m = 0
+    for j in range(nb):
+        d_best, e_best, hit = int(match[j]), int(best[j]), match[j] >= 0
+        for p in range(ptr[j], ptr[j + 1]):
+            d = idx[p]
+            if kept[d]:
+                hit = True
+                c, e = n0 + int(rank[d]), eq[p]
+                if e > e_best or (e == e_best and c < d_best):
+                    d_best, e_best = c, e
+        if hit:
+            match[j], best[j] = d_best, e_best
+        else:
+            kept[j], rank[j], m = True, m, m + 1
+            match[j], best[j] = -1, -1
+    if m:
+        lsh.insert(bsig[torch.from_numpy(kept).to(bsig.device)])
+    return kept, match.astype(np.int32), best.astype(np.int32)
+
+
+def c3_insert_unique(lsh, tok, perms, nb, min_jaccard=0.8, rounds=3):
+    """GpuLSH.insert_unique(min_jaccard) of nb fresh documents (c3_unique_batch) against the C3 index, beside the flow it
+    replaces (two_step_unique), wall-clock from a synchronised device to the result, the two alternating.  After each
+    call the kept rows are removed again and the index compacted (not timed).  In the same run the kept masks, matches
+    and the indexes after either flow (query of a sample of the batch) are compared."""
+    n, k = len(lsh), lsh.h
+    t = tok.shape[1]
+    g = torch.Generator(device="cuda").manual_seed(13)
+    btok = c3_unique_batch(tok, nb, g)
+    boff = torch.arange(0, (nb + 1) * t, t, dtype=torch.int64, device="cuda")
+    bsig = dsk.engine.bulk_signatures_device(btok.view(-1), boff, nb * t, perms)
+    probe = bsig[::25]
+
+    def undo():
+        if len(lsh) > n:
+            lsh.remove(torch.arange(n, len(lsh), device="cuda"))
+            lsh.compact()
+
+    def timed(fn):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        res = fn()
+        torch.cuda.synchronize()
+        return (time.perf_counter() - t0) * 1e3, res
+
+    calls = {"insert_unique": lambda: lsh.insert_unique(bsig, min_jaccard),
+             "two_step": lambda: two_step_unique(lsh, bsig, min_jaccard)}
+    times = {name: [] for name in calls}
+    results, states = {}, {}
+    for rep in range(rounds + 1):                          # the first round warms both flows up
+        for name, fn in calls.items():
+            ms, res = timed(fn)
+            if rep:
+                times[name].append(ms)
+            results[name] = res
+            p, x = lsh.query(probe)
+            states[name] = (p, [sorted(x[p[q]:p[q + 1]].tolist()) for q in range(len(p) - 1)], len(lsh))
+            undo()
+    (k1, m1, e1), (k2, m2, e2) = results["insert_unique"], results["two_step"]
+    out = {"iu_batch": nb, "iu_min_jaccard": min_jaccard, "iu_index_docs": n, "iu_kept": int(k1.sum()),
+           "iu_dropped_by_index": int(((m1 >= 0) & (m1 < n)).sum()), "iu_dropped_by_batch": int((m1 >= n).sum()),
+           "iu_kept_equal": bool(np.array_equal(k1, k2)),
+           "iu_match_eq_equal": bool(np.array_equal(m1, m2) and np.array_equal(e1, e2)),
+           "iu_index_after_equal": bool(np.array_equal(states["insert_unique"][0], states["two_step"][0]) and
+                                        states["insert_unique"][1:] == states["two_step"][1:])}
+    for name, ts in times.items():
+        out["iu_%s_ms" % name] = ts
+    out.update({"iu_" + key: v for key, v in gpu_card().items()})
+    return out
+
+
 def c4(n_vec, dim=4096, ss=128):
     gen = dsk.WeightedMinHashGenerator(dim, ss, 1)
     g = torch.Generator(device="cuda").manual_seed(4)
@@ -364,10 +474,14 @@ if __name__ == "__main__":
     ap.add_argument("--c3-query-jaccard", action="store_true",
                     help="also time GpuLSH.query_jaccard / query_best for 100k fresh documents against the C3 index, beside "
                          "query() and the two-step flow they replace, and compare their outputs")
+    ap.add_argument("--c3-insert-unique", action="store_true",
+                    help="also time GpuLSH.insert_unique(0.8) of 100k fresh documents against the C3 index, beside the "
+                         "flow it replaces (query_best, a temporary index's candidate_pairs, a host greedy loop, insert), "
+                         "and compare their outputs")
     a = ap.parse_args()
     if a.c3_docs > 0:
         print(json.dumps(c3(a.c3_docs, fused_leg=a.c3_fused, dedup_leg=a.c3_dedup, remove_leg=a.c3_remove,
-                            query_jaccard_leg=a.c3_query_jaccard)), flush=True)
+                            query_jaccard_leg=a.c3_query_jaccard, insert_unique_leg=a.c3_insert_unique)), flush=True)
     for fn, arg in ((c4, a.c4_vecs), (c5, a.c5_rows)):
         if arg > 0:
             print(json.dumps(fn(arg)), flush=True)
