@@ -16,7 +16,7 @@ from .b_bit_minhash import bBitMinHash  # noqa: E402
 from .weighted_minhash import WeightedMinHash, WeightedMinHashGenerator  # noqa: E402
 from .lsh import GpuLSH, MinHashLSH, MinHashLSHDeletionSession, MinHashLSHInsertionSession  # noqa: E402
 from .lshforest import GpuLSHForest, MinHashLSHForest  # noqa: E402
-from .lshensemble import MinHashLSHEnsemble  # noqa: E402
+from .lshensemble import GpuLSHEnsemble, MinHashLSHEnsemble  # noqa: E402
 from .lsh_bloom import MinHashLSHBloom  # noqa: E402
 from . import codec, distributed, engine  # noqa: E402
 
@@ -24,5 +24,5 @@ from . import codec, distributed, engine  # noqa: E402
 WeightedMinHashLSH = MinHashLSH
 
 __version__ = "0.1.0"
-__all__ = ["MinHash", "LeanMinHash", "bBitMinHash", "WeightedMinHash", "WeightedMinHashGenerator", "MinHashLSH", "GpuLSH", "MinHashLSHForest", "GpuLSHForest", "MinHashLSHEnsemble", "MinHashLSHBloom", "MinHashLSHBloom",
+__all__ = ["MinHash", "LeanMinHash", "bBitMinHash", "WeightedMinHash", "WeightedMinHashGenerator", "MinHashLSH", "GpuLSH", "MinHashLSHForest", "GpuLSHForest", "MinHashLSHEnsemble", "GpuLSHEnsemble", "MinHashLSHBloom", "MinHashLSHBloom",
            "WeightedMinHashLSH", "MinHashLSHInsertionSession", "MinHashLSHDeletionSession", "sha1_hash32", "sha1_hash64", "xxh32_hash32", "murmur3_hash32", "engine", "codec", "distributed"]

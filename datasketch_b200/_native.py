@@ -68,6 +68,13 @@ SIGNATURES = {
     "dsk_lsh_unique_count": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_size_t, c_void_p, c_void_p]),
     "dsk_lsh_unique_commit": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_size_t, c_void_p, c_void_p,
                                       c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_int64), c_void_p]),
+    "dsk_lsh_ensemble_create": (c_int, [c_int, c_int, c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(c_void_p)]),
+    "dsk_lsh_ensemble_destroy": (None, [c_void_p]),
+    "dsk_lsh_ensemble_size": (c_int, [c_void_p, ctypes.POINTER(c_int64)]),
+    "dsk_lsh_ensemble_index_bytes": (ctypes.c_size_t, [c_void_p, c_int64]),
+    "dsk_lsh_ensemble_index": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "dsk_lsh_ensemble_query_count": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
+    "dsk_lsh_ensemble_query_fill": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dsk_lsh_remove": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "dsk_lsh_alive": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     "dsk_lsh_compact_workspace_size": (ctypes.c_size_t, [c_void_p]),

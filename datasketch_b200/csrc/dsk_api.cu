@@ -173,6 +173,12 @@ struct dsk_lsh {
     } unique{};
 };
 
+struct dsk_lsh_ensemble {
+    int device = 0;
+    EnsembleDev dev{};    // device buffers allocated by dsk_lsh_ensemble_index
+    int64_t n_sets = 0;   // 0 until the index is built
+};
+
 extern "C" {
 
 int dsk_version(void) { return DSK_VERSION; }
@@ -1119,6 +1125,209 @@ int dsk_lsh_unique_commit(dsk_lsh *ix, const uint32_t *d_sig, int64_t n, int min
     ix->n_docs += m;
     ++ix->changes;
     *h_inserted = m;
+    return DSK_OK;
+}
+
+// ---- MinHashLSHEnsemble ------------------------------------------------------------------------------------------------
+static int64_t ensemble_cap_slots(int64_t n) {
+    int64_t c = 2;
+    while (c < 2 * n) c <<= 1;
+    return c;
+}
+
+static void ensemble_free(dsk_lsh_ensemble *e);
+
+size_t dsk_lsh_ensemble_index_bytes(const dsk_lsh_ensemble *e, int64_t n_sets) {
+    if (!e || n_sets <= 0) return 0;
+    const EnsembleDev &en = e->dev;
+    size_t bytes = (size_t)n_sets * en.tab[0].k * 4 + (size_t)n_sets * 4 + (size_t)(en.num_part + 1) * 8;
+    for (int t = 0; t < en.n_tabs; ++t)
+        bytes += (size_t)en.tab[t].b * ((size_t)ensemble_cap_slots(n_sets) * 16 + (size_t)n_sets * 4);
+    return bytes;
+}
+
+int dsk_lsh_ensemble_create(int num_perm, int num_part, const int32_t *h_b, const int32_t *h_r, int n_params, int device,
+                            dsk_lsh_ensemble **out) {
+    if (!out || !h_b || !h_r || num_perm < 2 || num_part < 1 || n_params < 1 || n_params > kEnsembleMaxParams) {
+        set_error("dsk_lsh_ensemble_create: need num_perm >= 2, num_part >= 1, 1 <= n_params <= %d and the (b, r) table",
+                  kEnsembleMaxParams);
+        return DSK_ERR_INVALID;
+    }
+    for (int i = 0; i < n_params; ++i) {
+        if (h_b[i] < 1 || h_r[i] < 1 || (int64_t)h_b[i] * h_r[i] > num_perm) {
+            set_error("dsk_lsh_ensemble_create: row %d of the (b, r) table needs b, r >= 1 and b*r <= num_perm (got b=%d r=%d "
+                      "num_perm=%d)", i, h_b[i], h_r[i], num_perm);
+            return DSK_ERR_INVALID;
+        }
+    }
+    DevInfo *d;
+    int rc = get_dev(device, &d);
+    if (rc) return rc;
+    dsk_lsh_ensemble *e = new (std::nothrow) dsk_lsh_ensemble();
+    if (!e) return DSK_ERR_NOMEM;
+    e->device = device;
+    EnsembleDev &en = e->dev;
+    en.num_part = num_part;
+    en.n_params = n_params;
+    for (int i = 0; i < n_params; ++i) {   // one table set per distinct r, in order of first appearance
+        int t = 0;
+        while (t < en.n_tabs && en.tab[t].r != h_r[i]) ++t;
+        if (t == en.n_tabs) {
+            LshDev &v = en.tab[en.n_tabs++];
+            v.k = num_perm;
+            v.r = h_r[i];
+            v.b = num_perm / h_r[i];
+        }
+        en.pb[i] = h_b[i];
+        en.pt[i] = t;
+    }
+    for (int t = en.n_tabs; t < kEnsembleMaxParams; ++t) en.tab[t].k = num_perm;
+    *out = e;
+    return DSK_OK;
+}
+
+static void ensemble_free(dsk_lsh_ensemble *e) {
+    int prev = 0;
+    cudaGetDevice(&prev);
+    cudaSetDevice(e->device);
+    EnsembleDev &en = e->dev;
+    if (en.tab[0].sig) cudaFree(en.tab[0].sig);
+    if (en.map) cudaFree(en.map);
+    if (en.part_start) cudaFree(en.part_start);
+    for (int t = 0; t < en.n_tabs; ++t) {
+        if (en.tab[t].slots) cudaFree(en.tab[t].slots);
+        if (en.tab[t].next) cudaFree(en.tab[t].next);
+        en.tab[t].sig = nullptr;
+        en.tab[t].slots = nullptr;
+        en.tab[t].next = nullptr;
+        en.tab[t].cap_docs = en.tab[t].cap_slots = 0;
+    }
+    en.map = nullptr;
+    en.part_start = nullptr;
+    e->n_sets = 0;
+    cudaSetDevice(prev);
+}
+
+void dsk_lsh_ensemble_destroy(dsk_lsh_ensemble *e) {
+    if (!e) return;
+    ensemble_free(e);
+    delete e;
+}
+
+int dsk_lsh_ensemble_size(const dsk_lsh_ensemble *e, int64_t *n_sets) {
+    if (!e) {
+        set_error("dsk_lsh_ensemble_size: null handle");
+        return DSK_ERR_INVALID;
+    }
+    if (n_sets) *n_sets = e->n_sets;
+    return DSK_OK;
+}
+
+int dsk_lsh_ensemble_index(dsk_lsh_ensemble *e, const uint32_t *d_sig, int64_t n, const int32_t *d_order,
+                           const int64_t *h_part_start, void *stream) {
+    if (!e) {
+        set_error("dsk_lsh_ensemble_index: null handle");
+        return DSK_ERR_INVALID;
+    }
+    if (e->n_sets > 0) {
+        set_error("dsk_lsh_ensemble_index: Cannot call index again on a non-empty index");
+        return DSK_ERR_INVALID;
+    }
+    if (n < 1 || n >= (1ll << 31)) {
+        set_error("dsk_lsh_ensemble_index: n must be in [1, 2^31) (got %lld)", (long long)n);
+        return DSK_ERR_INVALID;
+    }
+    if (!d_sig || !d_order || !h_part_start) {
+        set_error("dsk_lsh_ensemble_index: null buffer");
+        return DSK_ERR_INVALID;
+    }
+    EnsembleDev &en = e->dev;
+    bool ok = h_part_start[0] == 0 && h_part_start[en.num_part] == n;
+    for (int p = 0; p < en.num_part && ok; ++p) ok = h_part_start[p] <= h_part_start[p + 1];
+    if (!ok) {
+        set_error("dsk_lsh_ensemble_index: h_part_start must rise from 0 to n over num_part + 1 = %d entries", en.num_part + 1);
+        return DSK_ERR_INVALID;
+    }
+    DevInfo *dev;
+    int rc = get_dev(e->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(e->device);
+    const int k = en.tab[0].k;
+    const int64_t cap = ensemble_cap_slots(n);
+    uint32_t *sig = nullptr;
+    cudaError_t err = cudaMalloc(&sig, (size_t)n * k * 4);
+    for (int t = 0; t < en.n_tabs; ++t) {
+        en.tab[t].sig = sig;
+        en.tab[t].cap_docs = n;
+        en.tab[t].cap_slots = cap;
+    }
+    if (err == cudaSuccess) err = cudaMalloc(&en.map, (size_t)n * 4);
+    if (err == cudaSuccess) err = cudaMalloc(&en.part_start, (size_t)(en.num_part + 1) * 8);
+    for (int t = 0; t < en.n_tabs && err == cudaSuccess; ++t) {
+        err = cudaMalloc(&en.tab[t].slots, (size_t)en.tab[t].b * cap * 16);
+        if (err == cudaSuccess) err = cudaMalloc(&en.tab[t].next, (size_t)en.tab[t].b * n * 4);
+    }
+    if (err == cudaSuccess)
+        err = cudaMemcpy(en.part_start, h_part_start, (size_t)(en.num_part + 1) * 8, cudaMemcpyHostToDevice);
+    if (err == cudaSuccess) err = ensemble_index(en, d_sig, d_order, n, dev->sm_count, (cudaStream_t)stream);
+    if (err != cudaSuccess) {   // nothing is kept: the handle is empty again and can index
+        cudaGetLastError();
+        const size_t need = dsk_lsh_ensemble_index_bytes(e, n);
+        int rc2 = cuda_fail(err, "dsk_lsh_ensemble_index");
+        if (err == cudaErrorMemoryAllocation)
+            set_error("dsk_lsh_ensemble_index: cannot allocate the %zu bytes of device memory an index of %lld sets needs",
+                      need, (long long)n);
+        ensemble_free(e);
+        return rc2;
+    }
+    e->n_sets = n;
+    return DSK_OK;
+}
+
+// handle, nq >= 0 and, when nq > 0, the query matrix, the selection table and every output buffer
+static int check_ensemble_query(const char *who, const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq,
+                                const int32_t *d_sel, bool bufs) {
+    if (!e) {
+        set_error("%s: null handle", who);
+        return DSK_ERR_INVALID;
+    }
+    if (nq < 0 || nq > INT64_MAX / e->dev.num_part) {
+        set_error("%s: nq must be >= 0 (got %lld)", who, (long long)nq);
+        return DSK_ERR_INVALID;
+    }
+    if (nq > 0 && (!d_qsig || !d_sel || !bufs)) {
+        set_error("%s: null buffer", who);
+        return DSK_ERR_INVALID;
+    }
+    return DSK_OK;
+}
+
+int dsk_lsh_ensemble_query_count(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int32_t *d_sel,
+                                 int64_t *d_counts, void *stream) {
+    int rc = check_ensemble_query("dsk_lsh_ensemble_query_count", e, d_qsig, nq, d_sel, d_counts != nullptr);
+    if (rc || nq == 0) return rc;
+    DevGuard guard(e->device);
+    if (e->n_sets == 0) {   // nothing indexed: no partition has an upper bound, no query has a candidate
+        DSK_CUDA(cudaMemsetAsync(d_counts, 0, (size_t)nq * e->dev.num_part * 8, (cudaStream_t)stream));
+        return DSK_OK;
+    }
+    DevInfo *dev;
+    rc = get_dev(e->device, &dev);
+    if (rc) return rc;
+    DSK_CUDA(ensemble_query(e->dev, d_qsig, nq, d_sel, d_counts, nullptr, nullptr, nullptr, dev->sm_count,
+                            (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_lsh_ensemble_query_fill(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int32_t *d_sel,
+                                const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq, void *stream) {
+    int rc = check_ensemble_query("dsk_lsh_ensemble_query_fill", e, d_qsig, nq, d_sel, d_ptr && d_idx);
+    if (rc || nq == 0 || e->n_sets == 0) return rc;
+    DevInfo *dev;
+    rc = get_dev(e->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(e->device);
+    DSK_CUDA(ensemble_query(e->dev, d_qsig, nq, d_sel, nullptr, d_ptr, d_idx, d_eq, dev->sm_count, (cudaStream_t)stream));
     return DSK_OK;
 }
 

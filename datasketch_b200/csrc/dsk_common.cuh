@@ -161,6 +161,20 @@ cudaError_t lsh_unique_resolve(const LshDev &ix, int64_t n_docs, const uint32_t 
 cudaError_t lsh_unique_insert(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int64_t m, void *ws,
                               int sm_count, cudaStream_t s);
 
+// ---- device-resident MinHashLSHEnsemble (lsh_kernels.cu) ----------------------------------------------------------------
+constexpr int kEnsembleMaxParams = 16;   // rows of the (b, r) table (the reference's has 10)
+struct EnsembleDev {
+    LshDev tab[kEnsembleMaxParams];      // one band-table set per distinct r (n_tabs of them), all with sig = the rows in size order
+    int32_t *map;                        // [n] set number (size order) -> the caller's row
+    int64_t *part_start;                 // [num_part + 1] partition p = set numbers [part_start[p], part_start[p + 1])
+    int num_part, n_params, n_tabs;
+    int pb[kEnsembleMaxParams], pt[kEnsembleMaxParams];   // (b, r) table row -> b, and the table set of its r
+};
+cudaError_t ensemble_index(const EnsembleDev &en, const uint32_t *rows, const int32_t *order, int64_t n, int sm_count,
+                           cudaStream_t s);
+cudaError_t ensemble_query(const EnsembleDev &en, const uint32_t *qsig, int64_t nq, const int32_t *sel, int64_t *counts,
+                           const int64_t *ptr, int32_t *idx, int32_t *eq, int sm_count, cudaStream_t s);
+
 cudaError_t launch_jaccard_pairs(const uint32_t *sig, int64_t n_rows, int k, const int64_t *ia, const int64_t *ib,
                                  int64_t m, int32_t *out, int sm_count, cudaStream_t s);
 

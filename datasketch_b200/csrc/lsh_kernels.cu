@@ -1046,3 +1046,206 @@ cudaError_t lsh_unique_insert(const LshDev &ix, int64_t n_docs, const uint32_t *
 }
 
 }  // namespace dsk
+
+// ---- MinHashLSHEnsemble: containment search over size partitions (lshensemble.py:189-249) ---------------------------------
+// The reference keeps num_part x |rs| MinHashLSH indexes: indexes[p][r] holds the sets of size partition p, banded as
+// (num_perm // r, r), and query(m, size) unions, over every partition p with an upper bound, the first b bands of
+// indexes[p][r] with (b, r) = params[searchsorted(xqs, upper_p / size)].  Here the N sets are numbered in size-sorted order,
+// so partition p is the range [part_start[p], part_start[p + 1]) of set numbers, and their rows are held once.  For each
+// distinct r there is one set of b_r = num_perm // r band tables over all N sets, keyed by (partition, band, r-tuple): the
+// fingerprint of ensemble_fp is band_fp's with the partition in the seed's high word, so a chain holds the members of one
+// reference bucket indexes[p][r].hashtables[band][H] (plus fingerprint collisions, which the tuple check and the partition
+// range drop).  map[d] translates set number d back to the caller's row.
+namespace dsk {
+
+__device__ __forceinline__ uint64_t ensemble_fp(const uint32_t *v, int r, int band, int part) {
+    uint64_t h = 0x9E3779B97F4A7C15ull ^ (uint64_t)band ^ ((uint64_t)(uint32_t)part << 32);
+    for (int q = 0; q < r; ++q) h = (h ^ v[q]) * 0xFF51AFD7ED558CCDull + 0x2545F4914F6CDD1Dull;
+    h = lsh_mix64(h);
+    return h == kEmptyKey ? h - 1 : h;
+}
+
+// the partition of set number d: the last p with part_start[p] <= d (empty partitions have part_start[p] == part_start[p+1])
+__device__ __forceinline__ int ensemble_part(const int64_t *part_start, int num_part, int64_t d) {
+    int lo = 0, hi = num_part;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(part_start + mid) <= d) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// thread <-> (set d, band): the claim and chain update of lsh_insert_kernel, with the partition-keyed fingerprint.  The rows
+// are in the table's storage already (gathered in size order), so they are only read.
+__global__ void __launch_bounds__(256) ensemble_insert_kernel(const LshDev ix, const int64_t *__restrict__ part_start,
+                                                              int num_part, int64_t n) {
+    const uint64_t mask = (uint64_t)ix.cap_slots - 1;
+    const int64_t n_pairs = n * ix.b;
+    for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n_pairs; p += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t d = p / ix.b;
+        const int band = (int)(p - d * ix.b);
+        const int part = ensemble_part(part_start, num_part, d);
+        const uint64_t fp = ensemble_fp(ix.sig + d * ix.k + band * ix.r, ix.r, band, part);
+        uint64_t *tab = ix.slots + (int64_t)band * ix.cap_slots * 2;
+        uint64_t slot = lsh_mix64(fp) & mask;
+        while (true) {
+            const unsigned long long prev = atomicCAS(reinterpret_cast<unsigned long long *>(tab + 2 * slot),
+                                                      (unsigned long long)kEmptyKey, (unsigned long long)fp);
+            if (prev == kEmptyKey || prev == fp) break;
+            slot = (slot + 1) & mask;
+        }
+        const int32_t old = atomicExch(reinterpret_cast<int32_t *>(tab + 2 * slot + 1), (int32_t)d);
+        ix.next[d * ix.b + band] = old;
+    }
+}
+
+enum { ENS_COUNT = 0, ENS_FILL = 1, ENS_FILL_EQ = 2 };
+
+// warp <-> item (query q, partition p) = q * num_part + p, lane <-> band < b (bands beyond 32 in further rounds), the query
+// row staged in shared memory.  sel[item] is the row of the (b, r) table for the pair (-1, or any value outside the table:
+// the partition is not queried).  Each lane probes its band's table of the chosen r with the partition-keyed fingerprint
+// and walks the chain to its next candidate d: inside p's range, the tuple really equal, and no earlier band j < band with
+// equal tuples (the first matching band among the first b emits it, the set union of MinHashLSH._query_b).  Then, as in
+// lsh_pairs_kernel, the warp writes the pending candidates of all lanes together (ENS_FILL_EQ first counts eq for each of
+// them over the two K-word rows).
+//   ENS_COUNT    counts[item] = number of candidates
+//   ENS_FILL     out_idx[ptr[item] ...) = map[d], in no particular order
+//   ENS_FILL_EQ  the same, and out_eq at the same positions = number of the K positions where the rows agree
+template <int MODE>
+__global__ void __launch_bounds__(256) ensemble_query_kernel(const EnsembleDev en, const uint32_t *__restrict__ qsig,
+                                                             int64_t nq, const int32_t *__restrict__ sel,
+                                                             int64_t *__restrict__ counts, const int64_t *__restrict__ ptr,
+                                                             int32_t *__restrict__ out_idx, int32_t *__restrict__ out_eq) {
+    DSK_DYNAMIC_SMEM_T(uint32_t, s_rows, 16);   // [warps][k]
+    const int lane = threadIdx.x & 31;
+    const int k = en.tab[0].k;
+    uint32_t *row = s_rows + (int64_t)(threadIdx.x >> 5) * k;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    const unsigned below = (1u << lane) - 1u;
+    const int64_t n_items = nq * en.num_part;
+    for (int64_t item = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < n_items; item += warps) {
+        const int64_t q = item / en.num_part;
+        const int part = (int)(item - q * en.num_part);
+        const int s = sel[item];
+        const int64_t lo = en.part_start[part], hi = en.part_start[part + 1];
+        if (s < 0 || s >= en.n_params || lo >= hi) {   // warp-uniform
+            if (MODE == ENS_COUNT && lane == 0) counts[item] = 0;
+            continue;
+        }
+        const int nb = en.pb[s];
+        const LshDev &ix = en.tab[en.pt[s]];
+        const uint64_t mask = (uint64_t)ix.cap_slots - 1;
+        const uint32_t *qrow = qsig + q * k;
+        __syncwarp();
+        for (int w = lane; w < k; w += 32) row[w] = qrow[w];
+        __syncwarp();
+        int64_t total = 0;   // candidates so far (the same in every lane)
+        for (int band0 = 0; band0 < nb; band0 += 32) {
+            const int band = band0 + lane;
+            const uint32_t *qt = row + band * ix.r;
+            int32_t d = -1;
+            if (band < nb) {
+                const uint64_t fp = ensemble_fp(qt, ix.r, band, part);
+                const uint64_t *tab = ix.slots + (int64_t)band * ix.cap_slots * 2;
+                uint64_t slot = lsh_mix64(fp) & mask;
+                while (true) {
+                    const uint64_t kk = tab[2 * slot];
+                    if (kk == fp) { d = *reinterpret_cast<const int32_t *>(tab + 2 * slot + 1); break; }
+                    if (kk == kEmptyKey) break;
+                    slot = (slot + 1) & mask;
+                }
+            }
+            while (true) {
+                int32_t cand = -1;
+                while (d >= 0) {
+                    const int32_t cur = d;
+                    d = ix.next[(int64_t)cur * ix.b + band];
+                    if (cur >= lo && cur < hi) {
+                        const uint32_t *drow = ix.sig + (int64_t)cur * k;
+                        if (tuple_eq(drow + band * ix.r, qt, ix.r)) {
+                            bool dup = false;
+                            for (int j = 0; j < band && !dup; ++j)
+                                dup = tuple_eq(drow + j * ix.r, row + j * ix.r, ix.r);
+                            if (!dup) { cand = cur; break; }
+                        }
+                    }
+                }
+                const unsigned pending = __ballot_sync(0xFFFFFFFFu, cand >= 0);
+                if (pending == 0u) break;
+                int eq = 0;
+                if (MODE == ENS_FILL_EQ) {
+                    for (unsigned m = pending; m; m &= m - 1u) {
+                        const int src = __ffs(m) - 1;
+                        const uint32_t *crow = ix.sig + (int64_t)__shfl_sync(0xFFFFFFFFu, cand, src) * k;
+                        int e = 0;
+                        for (int w = lane; w < k; w += 32) e += crow[w] == row[w];
+#pragma unroll
+                        for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xFFFFFFFFu, e, o);
+                        if (lane == src) eq = e;
+                    }
+                }
+                if (MODE != ENS_COUNT && cand >= 0) {
+                    const int64_t pos = ptr[item] + total + __popc(pending & below);
+                    out_idx[pos] = en.map[cand];
+                    if (MODE == ENS_FILL_EQ) out_eq[pos] = eq;
+                }
+                total += __popc(pending);
+            }
+        }
+        if (MODE == ENS_COUNT && lane == 0) counts[item] = total;
+    }
+}
+
+// Gathers the n rows into size order (sig[t] = rows[order[t]]), copies order as the map, and fills every table set.
+cudaError_t ensemble_index(const EnsembleDev &en, const uint32_t *rows, const int32_t *order, int64_t n, int sm_count,
+                           cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    const LshDev &t0 = en.tab[0];
+    auto grid_of = [&](int64_t work) {
+        int64_t g = (work + 255) / 256;
+        return (unsigned)(g > (int64_t)sm_count * 8 ? (int64_t)sm_count * 8 : (g < 1 ? 1 : g));
+    };
+    DSK_LAUNCH(compact_gather_kernel, grid_of(n * 32), 256, 0, s, rows, t0.k, order, (int64_t)0, n, t0.sig);
+    cudaError_t e = cudaMemcpyAsync(en.map, order, (size_t)n * 4, cudaMemcpyDeviceToDevice, s);
+    for (int t = 0; t < en.n_tabs && e == cudaSuccess; ++t) {
+        const LshDev &ix = en.tab[t];
+        e = cudaMemsetAsync(ix.slots, 0xFF, (size_t)ix.b * ix.cap_slots * 16, s);   // empty key, head -1
+        if (e != cudaSuccess) break;
+        DSK_LAUNCH(ensemble_insert_kernel, grid_of(n * ix.b), 256, 0, s, ix, (const int64_t *)en.part_start, en.num_part, n);
+        e = cudaGetLastError();
+    }
+    return e;
+}
+
+// counts != nullptr: counts[item] for the nq * num_part items; else the fill of idx (and eq, if not null) at ptr[item].
+cudaError_t ensemble_query(const EnsembleDev &en, const uint32_t *qsig, int64_t nq, const int32_t *sel, int64_t *counts,
+                           const int64_t *ptr, int32_t *idx, int32_t *eq, int sm_count, cudaStream_t s) {
+    const int64_t n_items = nq * en.num_part;
+    if (n_items <= 0) return cudaSuccess;
+    const int k = en.tab[0].k;
+    int w = 8;
+    while (w > 1 && (size_t)w * k * 4 > 48 * 1024) w >>= 1;
+    const size_t smem = (size_t)w * k * 4;
+    int64_t g = (n_items + w - 1) / w;
+    if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
+    const unsigned grid = (unsigned)g;
+    cudaError_t e;
+    if (counts) {
+        e = cudaFuncSetAttribute(ensemble_query_kernel<ENS_COUNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        DSK_LAUNCH(ensemble_query_kernel<ENS_COUNT>, grid, 32 * w, smem, s, en, qsig, nq, sel, counts, nullptr, nullptr,
+                   nullptr);
+    } else if (eq) {
+        e = cudaFuncSetAttribute(ensemble_query_kernel<ENS_FILL_EQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        DSK_LAUNCH(ensemble_query_kernel<ENS_FILL_EQ>, grid, 32 * w, smem, s, en, qsig, nq, sel, nullptr, ptr, idx, eq);
+    } else {
+        e = cudaFuncSetAttribute(ensemble_query_kernel<ENS_FILL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        DSK_LAUNCH(ensemble_query_kernel<ENS_FILL>, grid, 32 * w, smem, s, en, qsig, nq, sel, nullptr, ptr, idx, nullptr);
+    }
+    return cudaGetLastError();
+}
+
+}  // namespace dsk

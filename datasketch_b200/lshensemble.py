@@ -13,6 +13,7 @@ What runs where:
 """
 from __future__ import annotations
 
+import ctypes
 import random
 import string
 import struct
@@ -120,24 +121,29 @@ def optimal_partitions(sizes, counts, num_part: int) -> List[Tuple[int, int]]:
 
 
 # ---- the index ------------------------------------------------------------------------------------------------
+def _check_args(threshold, num_perm, num_part, m, weights) -> None:
+    """The constructor's argument checks (lshensemble.py:120-133)."""
+    if threshold > 1.0 or threshold < 0.0:
+        raise ValueError("threshold must be in [0.0, 1.0]")
+    if num_perm < 2:
+        raise ValueError("Too few permutation functions")
+    if num_part < 1:
+        raise ValueError("num_part must be at least 1")
+    if m < 2 or m > num_perm:
+        raise ValueError("m must be in the range of [2, num_perm]")
+    if any(w < 0.0 or w > 1.0 for w in weights):
+        raise ValueError("Weight must be in [0.0, 1.0]")
+    if sum(weights) != 1.0:
+        raise ValueError("Weights must sum to 1.0")
+
+
 class MinHashLSHEnsemble:
     """LSH Ensemble for containment queries (constructor contract of lshensemble.py:108-153)."""
 
     def __init__(self, threshold: float = 0.9, num_perm: int = 128, num_part: int = 16, m: int = 8,
                  weights: Tuple[float, float] = (0.5, 0.5), storage_config: Optional[dict] = None,
                  prepickle: Optional[bool] = None) -> None:
-        if threshold > 1.0 or threshold < 0.0:
-            raise ValueError("threshold must be in [0.0, 1.0]")
-        if num_perm < 2:
-            raise ValueError("Too few permutation functions")
-        if num_part < 1:
-            raise ValueError("num_part must be at least 1")
-        if m < 2 or m > num_perm:
-            raise ValueError("m must be in the range of [2, num_perm]")
-        if any(w < 0.0 or w > 1.0 for w in weights):
-            raise ValueError("Weight must be in [0.0, 1.0]")
-        if sum(weights) != 1.0:
-            raise ValueError("Weights must sum to 1.0")
+        _check_args(threshold, num_perm, num_part, m, weights)
         self.threshold = threshold
         self.h = num_perm
         self.m = m
@@ -224,3 +230,218 @@ class MinHashLSHEnsemble:
 
     def is_empty(self) -> bool:
         return all(all(index[r].is_empty() for r in index) for index in self.indexes)
+
+
+# ---- device-resident index ------------------------------------------------------------------------------------
+def _partition_ranges(sorted_sizes: np.ndarray, uppers: list) -> np.ndarray:
+    """``start[0..num_part]``: the reference's walk over the size-sorted sets (lshensemble.py:216-228) -- a set whose size
+    exceeds the current partition's upper bound moves the walk ONE partition on -- as ranges of sorted set numbers.
+    Equal sizes form a run; inside a run the walk can only move while the size exceeds the current bound, so each run is
+    handled in a few steps."""
+    n_part = len(uppers)
+    start = np.zeros(n_part + 1, dtype=np.int64)
+    vals, first = np.unique(sorted_sizes, return_index=True)
+    ends = np.append(first[1:], len(sorted_sizes))
+    curr = 0
+    for v, a, e in zip(vals.tolist(), first.tolist(), ends.tolist()):
+        while a < e and v > uppers[curr]:   # this set opens the next partition
+            curr += 1
+            start[curr] = a
+            a += 1
+    start[curr + 1:] = len(sorted_sizes)
+    return start
+
+
+def _index_plan(sizes: np.ndarray, num_part: int):
+    """Host side of ``GpuLSHEnsemble.index`` for set sizes ``int64[N]``: ``(lowers, uppers, order, start)`` -- the
+    reference's partition bounds over ``Counter(sizes)`` (None for the unused trailing partitions), the stable size order
+    (``order[t]`` = the row that becomes set number t, as ``entries.sort(key=size)``) and the partitions as ranges of
+    set numbers."""
+    vals, counts = np.unique(sizes, return_counts=True)      # = sorted(Counter(sizes).most_common())
+    lowers, uppers = [None] * num_part, [None] * num_part
+    for i, (lower, upper) in enumerate(optimal_partitions(vals, counts, num_part)):
+        lowers[i], uppers[i] = lower, upper
+    order = np.argsort(sizes, kind="stable")
+    return lowers, uppers, order, _partition_ranges(sizes[order], uppers)
+
+
+def _selection(xqs: np.ndarray, n_params: int, uppers: list, start: np.ndarray, sizes) -> np.ndarray:
+    """``int32[Q, num_part]``: the row of the (b, r) table each query uses in each partition -- ``_get_optimal_param(upper,
+    size)``'s ``searchsorted(xqs, float(upper) / float(size), side="left")`` clamped to the last row, in float64 as
+    there -- or -1 where the partition has no upper bound or no sets."""
+    sizes = np.asarray(sizes, dtype=np.int64).reshape(-1)
+    sel = np.full((len(sizes), len(uppers)), -1, dtype=np.int32)
+    for p, u in enumerate(uppers):
+        if u is None or start[p] == start[p + 1]:
+            continue
+        i = np.searchsorted(xqs, float(u) / sizes.astype(np.float64), side="left")
+        sel[:, p] = np.minimum(i, n_params - 1)
+    return sel
+
+
+class GpuLSHEnsemble:
+    """Device-resident ``MinHashLSHEnsemble``: containment search ("which indexed sets contain most of this query set")
+    over whole signature matrices.
+
+    The constructor's arguments, checks, ``params`` / ``xqs`` (the (b, r) table) and, after ``index``, ``lowers`` /
+    ``uppers`` (the size partitions) are the host class's.  ``index(sig, sizes)`` takes the N sets as the rows of a
+    signature matrix; ``query(sig, sizes)`` returns CSR arrays ``(ptr, idx)`` whose ``idx[ptr[q]:ptr[q+1]]`` are, as a
+    set, ``MinHashLSHEnsemble.query(m_q, size_q)`` on the same data, given as row numbers of the ``index`` call.
+
+    On the device the rows are held once, in size order, so each partition is a range of set numbers; for each distinct r
+    of the table one set of ``num_perm // r`` band tables is keyed by (partition, band, r-tuple).  Device memory, in
+    bytes, with ``cap`` the power of two >= 2N: ``4*K*N + 4*N + sum over distinct r of (K // r) * (16*cap + 4*N)``
+    (``dsk_lsh_ensemble_index_bytes``)."""
+
+    def __init__(self, threshold: float = 0.9, num_perm: int = 128, num_part: int = 16, m: int = 8,
+                 weights: Tuple[float, float] = (0.5, 0.5), device: int = 0) -> None:
+        _check_args(threshold, num_perm, num_part, m, weights)
+        self.threshold = threshold
+        self.h = num_perm
+        self.m = m
+        self.num_part = num_part
+        self.device = device
+        MinHashLSHEnsemble._init_optimal_params(self, weights)   # self.xqs, self.params
+        self.lowers: list = [None] * num_part
+        self.uppers: list = [None] * num_part
+        self.keys: Optional[list] = None
+        self._keyset: Optional[set] = None
+        self._start = np.zeros(num_part + 1, dtype=np.int64)
+        from . import _native as nv
+        nv.require_device(device)
+        b = np.ascontiguousarray(self.params[:, 0], dtype=np.int32)
+        r = np.ascontiguousarray(self.params[:, 1], dtype=np.int32)
+        h = ctypes.c_void_p()
+        nv.check(nv.load().dsk_lsh_ensemble_create(num_perm, num_part, b.ctypes.data, r.ctypes.data, len(b), device,
+                                                   ctypes.byref(h)))
+        self._h = h
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) is not None:
+                from . import _native as nv
+                nv.load().dsk_lsh_ensemble_destroy(self._h)
+                self._h = None
+        except Exception:  # noqa: BLE001
+            pass
+
+    _get_optimal_param = MinHashLSHEnsemble._get_optimal_param
+
+    def __len__(self) -> int:
+        from . import _native as nv
+        n = ctypes.c_int64()
+        nv.check(nv.load().dsk_lsh_ensemble_size(self._h, ctypes.byref(n)))
+        return int(n.value)
+
+    def is_empty(self) -> bool:
+        return len(self) == 0
+
+    def __contains__(self, key: Hashable) -> bool:
+        if self._keyset is not None:
+            return key in self._keyset
+        return isinstance(key, (int, np.integer)) and 0 <= key < len(self)
+
+    def _dev_sig(self, sig):
+        import torch
+        from .lsh import _signature_matrix
+        if isinstance(sig, np.ndarray):
+            sig = torch.from_numpy(_signature_matrix(sig).view(np.int32)).cuda(self.device)
+        if sig.dim() != 2 or sig.shape[1] != self.h:
+            raise ValueError("Expecting minhash with length %d, got %d" % (self.h, sig.shape[-1]))
+        if sig.element_size() != 4:
+            raise TypeError("GpuLSHEnsemble takes the 32-bit signature matrix")
+        return sig.contiguous()
+
+    @staticmethod
+    def _sizes(sizes, n: int) -> np.ndarray:
+        s = np.asarray(sizes.cpu() if hasattr(sizes, "cpu") else sizes).reshape(-1)
+        if s.size and s.dtype.kind not in "iu":
+            raise TypeError("set sizes must be integers")
+        s = s.astype(np.int64)
+        if len(s) != n:
+            raise ValueError("sizes must hold one size per row of sig (%d), got %d" % (n, len(s)))
+        return s
+
+    def index(self, sig, sizes, keys: Optional[Iterable[Hashable]] = None) -> None:
+        """Index the N sets given as the rows of ``sig`` ([N, K] uint32; numpy or CUDA tensor) with their sizes
+        (``int64[N]``, each > 0) and, optionally, one key per row.  Callable once, like the reference's ``index``; set j
+        is row j of this call.  Raises ``ValueError`` as the reference does for a second call, no sets and a size <= 0,
+        and for mismatched lengths or a wrong K; ``MemoryError`` if the device memory cannot be allocated, after which
+        the object is still empty and can index."""
+        import torch
+        from . import _native as nv
+        if not self.is_empty():
+            raise ValueError("Cannot call index again on a non-empty index")
+        n = int(sig.shape[0]) if sig.ndim == 2 else -1
+        if n == 0:
+            raise ValueError("entries is empty")
+        d_sig = self._dev_sig(sig)
+        sizes = self._sizes(sizes, n)
+        if np.any(sizes <= 0):
+            raise ValueError("Set size must be positive")
+        if keys is not None:
+            keys = list(keys)
+            if len(keys) != n:
+                raise ValueError("keys must hold one key per row of sig (%d), got %d" % (n, len(keys)))
+        if n >= 1 << 31:
+            raise ValueError("an index holds fewer than 2^31 sets")
+        lowers, uppers, order, start = _index_plan(sizes, self.num_part)
+        d_order = torch.from_numpy(order.astype(np.int32)).to(d_sig.device)
+        with torch.cuda.device(self.device):
+            nv.check(nv.load().dsk_lsh_ensemble_index(self._h, d_sig.data_ptr(), n, d_order.data_ptr(), start.ctypes.data,
+                                                      torch.cuda.current_stream().cuda_stream))
+        self.lowers, self.uppers, self._start = lowers, uppers, start
+        if keys is not None:
+            self.keys, self._keyset = keys, set(keys)
+
+    def selection(self, sizes) -> np.ndarray:
+        """``int32[Q, num_part]``: the row of ``params`` each query size uses in each partition (``_get_optimal_param``),
+        -1 where the partition has no upper bound or no sets."""
+        return _selection(self.xqs, len(self.params), self.uppers, self._start, sizes)
+
+    def query(self, sig, sizes, with_eq: bool = False, to_host: bool = True):
+        """Containment candidates of every row of ``sig`` with its set size (each > 0): ``(ptr int64[Q+1], idx
+        int32[M])``, plus ``eq int32[M]`` when ``with_eq``.
+
+        ``idx[ptr[q]:ptr[q+1]]`` lists each candidate once, unordered, as a row number of the ``index`` call; as a set it is
+        ``MinHashLSHEnsemble.query(m_q, size_q)``: over every partition p with an upper bound, with ``(b, r) =
+        params[selection(size_q)[p]]``, the sets of p that share the query's r-tuple in one of the first b bands of the
+        ``(num_perm // r, r)`` banding.  ``eq`` is the number of the ``num_perm`` positions where the query row and the
+        candidate's row agree (``eq / num_perm`` is ``MinHash.jaccard``): with the two sizes it estimates containment."""
+        import torch
+        from . import _native as nv
+        d_q = self._dev_sig(sig)
+        nq = int(d_q.shape[0])
+        sizes = self._sizes(sizes, nq)
+        if np.any(sizes <= 0):
+            raise ValueError("Set size must be positive")
+        dev = d_q.device
+        lib = nv.load()
+        items = nq * self.num_part
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream().cuda_stream
+            sel = torch.from_numpy(self.selection(sizes)).to(dev)
+            counts = torch.empty((max(items, 1),), dtype=torch.int64, device=dev)
+            iptr = torch.empty((items + 1,), dtype=torch.int64, device=dev)
+            scratch = torch.empty((items // 1024 + 2,), dtype=torch.int64, device=dev)
+            nv.check(lib.dsk_lsh_ensemble_query_count(self._h, d_q.data_ptr(), nq, sel.data_ptr(), counts.data_ptr(), st))
+            nv.check(lib.dsk_exclusive_scan(counts.data_ptr(), items, iptr.data_ptr(), scratch.data_ptr(), st))
+            total = int(iptr[items].item())
+            idx = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
+            eq = torch.empty((max(total, 1),), dtype=torch.int32, device=dev) if with_eq else None
+            nv.check(lib.dsk_lsh_ensemble_query_fill(self._h, d_q.data_ptr(), nq, sel.data_ptr(), iptr.data_ptr(),
+                                                     idx.data_ptr(), eq.data_ptr() if with_eq else None, st))
+            ptr = iptr[::self.num_part].contiguous()
+            out = (ptr, idx[:total]) + ((eq[:total],) if with_eq else ())
+        if to_host:
+            return tuple(x.cpu().numpy() for x in out)
+        return out
+
+    def query_keys(self, sig, sizes) -> List[list]:
+        """Like ``GpuLSH.query_keys``: per query, the list of keys (or row numbers, without keys) of its candidates."""
+        ptr, idx = self.query(sig, sizes)
+        out = []
+        for q in range(len(ptr) - 1):
+            ids = idx[ptr[q]:ptr[q + 1]]
+            out.append([self.keys[i] for i in ids] if self.keys is not None else ids.tolist())
+        return out

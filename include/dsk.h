@@ -316,6 +316,51 @@ DSK_API int dsk_lsh_unique_count(const dsk_lsh *ix, const uint32_t *d_sig, int64
 DSK_API int dsk_lsh_unique_commit(dsk_lsh *ix, const uint32_t *d_sig, int64_t n, int min_count, void *d_ws, size_t ws_bytes,
                                   const int64_t *d_ptr, int32_t *d_pidx, int32_t *d_peq, uint8_t *d_kept, int32_t *d_match,
                                   int32_t *d_eq, int64_t *h_inserted, void *stream);
+/* ---- device-resident MinHashLSHEnsemble (containment search) -------------------------------------------------------
+ * Replaces MinHashLSHEnsemble.index / query over dict storage (datasketch/lshensemble.py:189-249): num_part x |rs|
+ * MinHashLSH indexes filled per set and walked per query in Python.  The host computes what is control logic there and
+ * passes it in: the (b, r) table params (lshensemble.py:155-166, 10 rows), the size partitions and, per query and
+ * partition, the row of that table the query uses.
+ *   dsk_lsh_ensemble_create  h_b / h_r: the n_params (<= 16) rows of the (b, r) table, b*r <= num_perm.  For each distinct
+ *                        r the index keeps one set of b_r = num_perm / r band tables, as the reference's
+ *                        MinHashLSH(params=(num_perm / r, r)).  Allocates no device memory.
+ *   dsk_lsh_ensemble_index  indexes the n sets of d_sig ([n, num_perm] u32), once (a second call is DSK_ERR_INVALID).
+ *                        d_order[t] (a permutation of 0..n-1) is the row of d_sig that becomes set number t: the rows in
+ *                        stable size order, as the reference's entries.sort(key=size).  h_part_start[0..num_part] (host
+ *                        memory, rising from 0 to n): partition p holds set numbers [h_part_start[p], h_part_start[p+1]).
+ *                        A set matches another in band j of table set r iff both are in the same partition and their
+ *                        r-tuples in band j are equal (the bucket indexes[p][r].hashtables[j][H] of the reference).  It
+ *                        allocates, synchronously, dsk_lsh_ensemble_index_bytes(n) bytes of device memory:
+ *                          4 * num_perm * n              the rows, once, in size order
+ *                        + 4 * n + 8 * (num_part + 1)    the map set number -> row of d_sig, the partition bounds
+ *                        + sum over distinct r of b_r * (16 * cap_slots + 4 * n),  cap_slots = the power of two >= 2n
+ *                        (e.g. threshold 0.5, num_perm 128, m 8: rs = {1, 2, 3, 5, 8}, sum b_r = 275, about 11 GB at 1M
+ *                        sets).  If it cannot, it returns DSK_ERR_NOMEM and the handle stays empty and usable.
+ *   dsk_lsh_ensemble_query_count  d_sel[q * num_part + p] = the row of the (b, r) table query q uses in partition p
+ *                        (lshensemble.py:162-166: searchsorted(xqs, upper_p / size_q) clamped to the last row), or -1 to
+ *                        skip the partition (upper bound None); any value outside [0, n_params) skips it too.  Writes
+ *                        d_counts[q * num_part + p] = the number of candidates of q in p: the sets of p that share the
+ *                        query's r-tuple in one of the first b bands of the (num_perm / r, r) banding (MinHashLSH._query_b).
+ *   dsk_exclusive_scan   of the nq * num_part counts into d_ptr (nq * num_part + 1 entries)
+ *   dsk_lsh_ensemble_query_fill  writes the candidates of item q * num_part + p, each once, unordered, as rows of the
+ *                        index call's d_sig, at d_idx[d_ptr[item] .. d_ptr[item + 1]); q's whole result is
+ *                        d_idx[d_ptr[q * num_part] .. d_ptr[(q + 1) * num_part]).  d_eq (may be NULL): at the same
+ *                        positions, the number of the num_perm positions where the query row and the set's row agree.
+ * Queries check the handle, nq >= 0 and, for nq > 0, every buffer; nq == 0 with null buffers is a valid no-op, and an
+ * index that was never built has no candidates.  Cost: one warp per (query, partition) probes b tables of one set and
+ * walks the chains it hits, reading the r-tuple of each member (and, with d_eq, both rows of each candidate). */
+typedef struct dsk_lsh_ensemble dsk_lsh_ensemble;
+DSK_API int dsk_lsh_ensemble_create(int num_perm, int num_part, const int32_t *h_b, const int32_t *h_r, int n_params,
+                                    int device, dsk_lsh_ensemble **out);
+DSK_API void dsk_lsh_ensemble_destroy(dsk_lsh_ensemble *e);
+DSK_API int dsk_lsh_ensemble_size(const dsk_lsh_ensemble *e, int64_t *n_sets);
+DSK_API size_t dsk_lsh_ensemble_index_bytes(const dsk_lsh_ensemble *e, int64_t n_sets);
+DSK_API int dsk_lsh_ensemble_index(dsk_lsh_ensemble *e, const uint32_t *d_sig, int64_t n, const int32_t *d_order,
+                                   const int64_t *h_part_start, void *stream);
+DSK_API int dsk_lsh_ensemble_query_count(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int32_t *d_sel,
+                                         int64_t *d_counts, void *stream);
+DSK_API int dsk_lsh_ensemble_query_fill(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int32_t *d_sel,
+                                        const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq, void *stream);
 DSK_API int dsk_lsh_remove(dsk_lsh *ix, const int32_t *d_docs, int64_t n, int64_t *d_status, void *stream);
 DSK_API int dsk_lsh_alive(const dsk_lsh *ix, const int32_t *d_docs, int64_t n, uint8_t *d_out, void *stream);
 DSK_API size_t dsk_lsh_compact_workspace_size(const dsk_lsh *ix);
