@@ -158,6 +158,7 @@ struct dsk_wmh {
 struct dsk_lsh {
     int device = 0;
     LshDev dev{};
+    int sw = 1;                    // words per sample: 1 (MinHash), 2 (weighted: (k, t) packed, dev.k / dev.r count words)
     int64_t n_docs = 0;
     uint32_t *removed = nullptr;   // removal bitmap, (cap_docs + 31) / 32 words: allocated by the first dsk_lsh_remove
     bool has_removals = false;     // a dsk_lsh_remove since the last compaction: the walks run their removal-aware kernels
@@ -664,11 +665,16 @@ int dsk_wmh_minhash(const dsk_wmh *g, const float *d_v, int64_t n, int64_t *d_ou
     return DSK_OK;
 }
 
-int dsk_lsh_create(int num_perm, int b, int r, int64_t capacity_docs, int device, dsk_lsh **out) {
-    int rc = check_bands("dsk_lsh_create", capacity_docs, num_perm, b, r);
+// num_perm samples of sw words each; b and r count samples
+static int lsh_create(const char *who, int num_perm, int sw, int b, int r, int64_t capacity_docs, int device, dsk_lsh **out) {
+    int rc = check_bands(who, capacity_docs, num_perm, b, r);
     if (rc) return rc;
     if (!out || capacity_docs <= 0 || capacity_docs >= (1ll << 31)) {
-        set_error("dsk_lsh_create: capacity_docs must be in [1, 2^31)");
+        set_error("%s: capacity_docs must be in [1, 2^31)", who);
+        return DSK_ERR_INVALID;
+    }
+    if (num_perm > INT32_MAX / sw) {
+        set_error("%s: num_perm must be at most %d (got %d)", who, INT32_MAX / sw, num_perm);
         return DSK_ERR_INVALID;
     }
     DevInfo *d;
@@ -677,6 +683,9 @@ int dsk_lsh_create(int num_perm, int b, int r, int64_t capacity_docs, int device
     dsk_lsh *ix = new (std::nothrow) dsk_lsh();
     if (!ix) return DSK_ERR_NOMEM;
     ix->device = device;
+    ix->sw = sw;
+    num_perm *= sw;
+    r *= sw;
     LshDev &v = ix->dev;
     v.k = num_perm; v.b = b; v.r = r; v.cap_docs = capacity_docs;
     v.cap_slots = 1024;
@@ -691,12 +700,20 @@ int dsk_lsh_create(int num_perm, int b, int r, int64_t capacity_docs, int device
     if (e == cudaSuccess) e = cudaMemset(v.slots, 0xFF, slots * 2 * sizeof(uint64_t));   // empty key, head = -1
     cudaSetDevice(prev);
     if (e != cudaSuccess) {
-        int rc2 = cuda_fail(e, "dsk_lsh_create");
+        int rc2 = cuda_fail(e, who);
         dsk_lsh_destroy(ix);
         return rc2;
     }
     *out = ix;
     return DSK_OK;
+}
+
+int dsk_lsh_create(int num_perm, int b, int r, int64_t capacity_docs, int device, dsk_lsh **out) {
+    return lsh_create("dsk_lsh_create", num_perm, 1, b, r, capacity_docs, device, out);
+}
+
+int dsk_lsh_create_weighted(int sample_size, int b, int r, int64_t capacity_docs, int device, dsk_lsh **out) {
+    return lsh_create("dsk_lsh_create_weighted", sample_size, 2, b, r, capacity_docs, device, out);
 }
 
 void dsk_lsh_destroy(dsk_lsh *ix) {
@@ -746,6 +763,10 @@ int dsk_lsh_insert_tokens(dsk_lsh *ix, const dsk_perm *perm, const void *d_token
                           const int64_t *d_offsets, int64_t n_docs, int64_t n_tokens, void *stream) {
     if (!ix || !perm || !d_offsets || n_docs < 0 || n_tokens < 0 || (n_tokens > 0 && !d_tokens)) {
         set_error("dsk_lsh_insert_tokens: bad arguments");
+        return DSK_ERR_INVALID;
+    }
+    if (ix->sw != 1) {
+        set_error("dsk_lsh_insert_tokens: the index holds weighted MinHash rows; tokens give MinHash rows");
         return DSK_ERR_INVALID;
     }
     if (perm->num_perm != ix->dev.k || perm->device != ix->device) {
@@ -847,8 +868,10 @@ static int check_self_join(const char *who, const dsk_lsh *ix, int min_count) {
         set_error("%s: null handle", who);
         return DSK_ERR_INVALID;
     }
-    if (min_count < 0 || min_count > ix->dev.k) {
-        set_error("%s: min_count must be in [0, num_perm=%d] (got %d)", who, ix->dev.k, min_count);
+    const int samples = ix->dev.k / ix->sw;   // eq counts samples
+    if (min_count < 0 || min_count > samples) {
+        set_error("%s: min_count must be in [0, %s=%d] (got %d)", who, ix->sw == 1 ? "num_perm" : "sample_size", samples,
+                  min_count);
         return DSK_ERR_INVALID;
     }
     return DSK_OK;
@@ -865,7 +888,7 @@ int dsk_lsh_pairs_count(const dsk_lsh *ix, int min_count, int64_t *d_counts, voi
     rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->n_docs, min_count, d_counts, nullptr, nullptr, nullptr, ix->walk_bitmap(), dev->sm_count,
+    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->sw, ix->n_docs, min_count, d_counts, nullptr, nullptr, nullptr, ix->walk_bitmap(), dev->sm_count,
                               (cudaStream_t)stream));
     return DSK_OK;
 }
@@ -882,7 +905,7 @@ int dsk_lsh_pairs_fill(const dsk_lsh *ix, int min_count, const int64_t *d_ptr, i
     rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->n_docs, min_count, nullptr, d_ptr, d_idx, d_eq, ix->walk_bitmap(), dev->sm_count,
+    DSK_CUDA(launch_lsh_pairs(ix->dev, ix->sw, ix->n_docs, min_count, nullptr, d_ptr, d_idx, d_eq, ix->walk_bitmap(), dev->sm_count,
                               (cudaStream_t)stream));
     return DSK_OK;
 }
@@ -898,7 +921,7 @@ int dsk_lsh_clusters(const dsk_lsh *ix, int min_count, int32_t *d_labels, void *
     rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(launch_lsh_clusters(ix->dev, ix->n_docs, min_count, d_labels, ix->walk_bitmap(), dev->sm_count,
+    DSK_CUDA(launch_lsh_clusters(ix->dev, ix->sw, ix->n_docs, min_count, d_labels, ix->walk_bitmap(), dev->sm_count,
                                  (cudaStream_t)stream));
     return DSK_OK;
 }
@@ -926,7 +949,7 @@ static int run_query_pairs(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq
     int rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(launch_lsh_query_pairs(ix->dev, d_qsig, nq, ix->n_docs, min_count, d_counts, d_ptr, d_idx, d_eq,
+    DSK_CUDA(launch_lsh_query_pairs(ix->dev, ix->sw, d_qsig, nq, ix->n_docs, min_count, d_counts, d_ptr, d_idx, d_eq,
                                     ix->walk_bitmap(), dev->sm_count, (cudaStream_t)stream));
     return DSK_OK;
 }
@@ -1071,6 +1094,10 @@ static int check_unique(const char *who, const dsk_lsh *ix, const uint32_t *d_si
                   who, need, ws_bytes);
         return DSK_ERR_INVALID;
     }
+    if (ix->sw == 2 && ((uintptr_t)d_sig & 7) != 0) {   // the batch walk reads a sample of these rows with one 8-byte load
+        set_error("%s: d_sig must be 8-byte aligned for a weighted index", who);
+        return DSK_ERR_ALIGN;
+    }
     return DSK_OK;
 }
 
@@ -1084,7 +1111,7 @@ int dsk_lsh_unique_count(const dsk_lsh *ix, const uint32_t *d_sig, int64_t n, in
     rc = get_dev(ix->device, &dev);
     if (rc) return rc;
     DevGuard guard(ix->device);
-    DSK_CUDA(lsh_unique_count(ix->dev, ix->n_docs, d_sig, n, min_count, d_ws, d_counts, ix->walk_bitmap(), dev->sm_count,
+    DSK_CUDA(lsh_unique_count(ix->dev, ix->sw, ix->n_docs, d_sig, n, min_count, d_ws, d_counts, ix->walk_bitmap(), dev->sm_count,
                               (cudaStream_t)stream));
     ix->unique = {true, d_sig, d_ws, n, min_count, ix->changes};
     return DSK_OK;
@@ -1113,7 +1140,7 @@ int dsk_lsh_unique_commit(dsk_lsh *ix, const uint32_t *d_sig, int64_t n, int min
     DevGuard guard(ix->device);
     const cudaStream_t s = (cudaStream_t)stream;
     int64_t m = 0;
-    DSK_CUDA(lsh_unique_resolve(ix->dev, ix->n_docs, d_sig, n, min_count, d_ws, d_ptr, d_pidx, d_peq, d_kept, d_match, d_eq,
+    DSK_CUDA(lsh_unique_resolve(ix->dev, ix->sw, ix->n_docs, d_sig, n, min_count, d_ws, d_ptr, d_pidx, d_peq, d_kept, d_match, d_eq,
                                 &m, dev->sm_count, s));
     *h_inserted = 0;
     if (ix->n_docs + m > ix->dev.cap_docs) {

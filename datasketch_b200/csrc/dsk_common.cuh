@@ -130,15 +130,17 @@ cudaError_t launch_lsh_query(const LshDev &ix, const uint32_t *qsig, int64_t nq,
                              const int64_t *ptr, int32_t *out, int fill, int sm_count, cudaStream_t s);   // nothing removed
 cudaError_t launch_exclusive_scan(const int64_t *in, int64_t n, int64_t *out, int64_t *scratch, cudaStream_t s);
 // self-join of the first n_docs documents (d < i, a band's tuple equal, eq >= min_count): per-document counts, or the fill
-// of idx / eq at ptr[i] (counts == nullptr); clusters: labels[i] = smallest document of i's component of the pair graph
-cudaError_t launch_lsh_pairs(const LshDev &ix, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
+// of idx / eq at ptr[i] (counts == nullptr); clusters: labels[i] = smallest document of i's component of the pair graph.
+// sw (here and below) = words per sample of the rows: 1 for MinHash, 2 for weighted MinHash (ix.k and ix.r then count
+// words, 2 per sample), where eq counts the samples whose two words both agree.
+cudaError_t launch_lsh_pairs(const LshDev &ix, int sw, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
                              int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s);
-cudaError_t launch_lsh_clusters(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels, const uint32_t *removed,
+cudaError_t launch_lsh_clusters(const LshDev &ix, int sw, int64_t n_docs, int min_count, int32_t *labels, const uint32_t *removed,
                                 int sm_count, cudaStream_t s);
 // the self-join's walk for nq query rows outside the index (every d < n_docs eligible): per-query counts of the kept
 // candidates; the fill of idx / eq at ptr[q] (counts == nullptr); or each query's best kept candidate at idx[q] / eq[q]
 // (counts == ptr == nullptr)
-cudaError_t launch_lsh_query_pairs(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count,
+cudaError_t launch_lsh_query_pairs(const LshDev &ix, int sw, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count,
                                    int64_t *counts, const int64_t *ptr, int32_t *idx, int32_t *eq, const uint32_t *removed,
                                    int sm_count, cudaStream_t s);
 // removal (bits of the bitmap) and compaction of the index
@@ -153,9 +155,9 @@ cudaError_t lsh_compact(const LshDev &ix, const uint32_t *removed, int64_t n_doc
 // insert_unique (the streaming dedup loop over a batch of n rows): workspace bytes; the batch table, stage A and the counts
 // of the earlier partners; the fill, resolution and matches (*m = kept rows, one synchronisation); the insert of the kept
 size_t lsh_unique_workspace_bytes(const LshDev &ix, int64_t n);
-cudaError_t lsh_unique_count(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
+cudaError_t lsh_unique_count(const LshDev &ix, int sw, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
                              int64_t *counts, const uint32_t *removed, int sm_count, cudaStream_t s);
-cudaError_t lsh_unique_resolve(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
+cudaError_t lsh_unique_resolve(const LshDev &ix, int sw, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
                                const int64_t *ptr, int32_t *pidx, int32_t *peq, uint8_t *kept, int32_t *match, int32_t *eq,
                                int64_t *m, int sm_count, cudaStream_t s);
 cudaError_t lsh_unique_insert(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int64_t m, void *ws,

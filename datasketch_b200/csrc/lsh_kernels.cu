@@ -390,7 +390,11 @@ enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2, QUERY_COUNT = 3, QUERY_
 //   QUERY_BEST   idx[i] / eq[i] = the kept partner with the largest eq, the smallest d among equal ones (-1 / -1: none).
 //                Each lane keeps its own best and a warp shuffle reduction picks the query's: no atomics.
 // In the PAIRS modes qsig and nq are unused and the code is the self-join's alone.
-template <int MODE, bool RM>
+// SW = words per sample.  SW = 1: MinHash rows, eq counts equal words.  SW = 2: weighted MinHash rows, sample s = words
+// 2s (k) and 2s + 1 (t), ix.k = 2 * sample_size and ix.r = 2 * r words; eq counts the samples whose two words are both
+// equal (WeightedMinHash.jaccard * sample_size), each read with one 8-byte load (rows of 2 * sample_size words stay 8-byte
+// aligned).  Bands, chains, tuple checks and the first-matching-band rule work on words and need no change.
+template <int MODE, bool RM, int SW = 1>
 __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t n_docs, int min_count,
                                                         int64_t *__restrict__ counts, const int64_t *__restrict__ ptr,
                                                         int32_t *__restrict__ out_idx, int32_t *__restrict__ out_eq,
@@ -454,7 +458,14 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
                         const int src = __ffs(m) - 1;
                         const uint32_t *crow = ix.sig + (int64_t)__shfl_sync(0xFFFFFFFFu, cand, src) * ix.k;
                         int e = 0;
-                        for (int w = lane; w < ix.k; w += 32) e += crow[w] == row[w];
+                        if constexpr (SW == 1) {
+                            for (int w = lane; w < ix.k; w += 32) e += crow[w] == row[w];
+                        } else {
+                            // a sample's two words as one 64-bit value: equal iff k and t are both equal
+                            const uint64_t *c2 = reinterpret_cast<const uint64_t *>(crow);
+                            const uint64_t *r2 = reinterpret_cast<const uint64_t *>(row);
+                            for (int w = lane; w < (ix.k >> 1); w += 32) e += c2[w] == r2[w];
+                        }
 #pragma unroll
                         for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xFFFFFFFFu, e, o);
                         if (lane == src) eq = e;
@@ -527,7 +538,7 @@ __global__ void __launch_bounds__(256) lsh_link_kernel(const LshDev ix, int64_t 
 
 // the pair walk's launch shape for `rows` staged rows (documents, or queries with M0 = QUERY_COUNT): up to 8 warps per
 // CTA, each with a K-word row in shared memory.  Allows that much shared memory to the modes M0, M0 + 1 and M0 + 2.
-template <bool RM, int M0 = PAIRS_COUNT>
+template <bool RM, int M0 = PAIRS_COUNT, int SW = 1>
 static cudaError_t pairs_shape(const LshDev &ix, int64_t rows, int sm_count, int *warps, unsigned *grid, size_t *smem) {
     int w = 8;
     while (w > 1 && (size_t)w * ix.k * 4 > 48 * 1024) w >>= 1;
@@ -536,41 +547,45 @@ static cudaError_t pairs_shape(const LshDev &ix, int64_t rows, int sm_count, int
     int64_t g = (rows + w - 1) / w;
     if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
     *grid = (unsigned)g;
-    cudaError_t e = cudaFuncSetAttribute(lsh_pairs_kernel<M0, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+    cudaError_t e = cudaFuncSetAttribute(lsh_pairs_kernel<M0, RM, SW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(lsh_pairs_kernel<M0 + 1, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+        e = cudaFuncSetAttribute(lsh_pairs_kernel<M0 + 1, RM, SW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(lsh_pairs_kernel<M0 + 2, RM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
+        e = cudaFuncSetAttribute(lsh_pairs_kernel<M0 + 2, RM, SW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem);
     return e;
 }
 
-template <bool RM>
+template <bool RM, int SW>
 static cudaError_t launch_pairs_t(const LshDev &ix, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
                                   int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s) {
     int warps;
     unsigned grid;
     size_t smem;
-    cudaError_t e = pairs_shape<RM>(ix, n_docs, sm_count, &warps, &grid, &smem);
+    cudaError_t e = pairs_shape<RM, PAIRS_COUNT, SW>(ix, n_docs, sm_count, &warps, &grid, &smem);
     if (e != cudaSuccess) return e;
     if (counts)
-        DSK_LAUNCH((lsh_pairs_kernel<PAIRS_COUNT, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr,
+        DSK_LAUNCH((lsh_pairs_kernel<PAIRS_COUNT, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr,
                    nullptr, nullptr, nullptr, removed, nullptr, 0);
     else
-        DSK_LAUNCH((lsh_pairs_kernel<PAIRS_FILL, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
+        DSK_LAUNCH((lsh_pairs_kernel<PAIRS_FILL, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
                    nullptr, removed, nullptr, 0);
     return cudaGetLastError();
 }
 
 // counts != nullptr: counts[i] for every document; else the fill of idx / eq at ptr[i].  removed != nullptr: the
-// removal-aware walk.
-cudaError_t launch_lsh_pairs(const LshDev &ix, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
+// removal-aware walk.  sw: words per sample of the index's rows (1 or 2).
+cudaError_t launch_lsh_pairs(const LshDev &ix, int sw, int64_t n_docs, int min_count, int64_t *counts, const int64_t *ptr,
                              int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s) {
     if (n_docs <= 0) return cudaSuccess;
-    if (removed) return launch_pairs_t<true>(ix, n_docs, min_count, counts, ptr, idx, eq, removed, sm_count, s);
-    return launch_pairs_t<false>(ix, n_docs, min_count, counts, ptr, idx, eq, nullptr, sm_count, s);
+    if (sw == 2) {
+        if (removed) return launch_pairs_t<true, 2>(ix, n_docs, min_count, counts, ptr, idx, eq, removed, sm_count, s);
+        return launch_pairs_t<false, 2>(ix, n_docs, min_count, counts, ptr, idx, eq, nullptr, sm_count, s);
+    }
+    if (removed) return launch_pairs_t<true, 1>(ix, n_docs, min_count, counts, ptr, idx, eq, removed, sm_count, s);
+    return launch_pairs_t<false, 1>(ix, n_docs, min_count, counts, ptr, idx, eq, nullptr, sm_count, s);
 }
 
-template <bool RM>
+template <bool RM, int SW>
 static cudaError_t launch_clusters_t(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels,
                                      const uint32_t *removed, int sm_count, cudaStream_t s) {
     int64_t grid = (n_docs + 255) / 256;
@@ -584,52 +599,61 @@ static cudaError_t launch_clusters_t(const LshDev &ix, int64_t n_docs, int min_c
         int warps;
         unsigned pg;
         size_t smem;
-        cudaError_t e = pairs_shape<RM>(ix, n_docs, sm_count, &warps, &pg, &smem);
+        cudaError_t e = pairs_shape<RM, PAIRS_COUNT, SW>(ix, n_docs, sm_count, &warps, &pg, &smem);
         if (e != cudaSuccess) return e;
-        DSK_LAUNCH((lsh_pairs_kernel<PAIRS_UNION, RM>), pg, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr,
+        DSK_LAUNCH((lsh_pairs_kernel<PAIRS_UNION, RM, SW>), pg, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr,
                    nullptr, nullptr, labels, removed, nullptr, 0);
     }
     DSK_LAUNCH(uf_flatten_kernel<RM>, (unsigned)grid, 256, 0, s, labels, n_docs, removed);
     return cudaGetLastError();
 }
 
-cudaError_t launch_lsh_clusters(const LshDev &ix, int64_t n_docs, int min_count, int32_t *labels, const uint32_t *removed,
-                                int sm_count, cudaStream_t s) {
+cudaError_t launch_lsh_clusters(const LshDev &ix, int sw, int64_t n_docs, int min_count, int32_t *labels,
+                                const uint32_t *removed, int sm_count, cudaStream_t s) {
     if (n_docs <= 0) return cudaSuccess;
-    if (removed) return launch_clusters_t<true>(ix, n_docs, min_count, labels, removed, sm_count, s);
-    return launch_clusters_t<false>(ix, n_docs, min_count, labels, nullptr, sm_count, s);
+    if (sw == 2) {
+        if (removed) return launch_clusters_t<true, 2>(ix, n_docs, min_count, labels, removed, sm_count, s);
+        return launch_clusters_t<false, 2>(ix, n_docs, min_count, labels, nullptr, sm_count, s);
+    }
+    if (removed) return launch_clusters_t<true, 1>(ix, n_docs, min_count, labels, removed, sm_count, s);
+    return launch_clusters_t<false, 1>(ix, n_docs, min_count, labels, nullptr, sm_count, s);
 }
 
-template <bool RM>
+template <bool RM, int SW>
 static cudaError_t launch_query_pairs_t(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count,
                                         int mode, int64_t *counts, const int64_t *ptr, int32_t *idx, int32_t *eq,
                                         const uint32_t *removed, int sm_count, cudaStream_t s) {
     int warps;
     unsigned grid;
     size_t smem;
-    cudaError_t e = pairs_shape<RM, QUERY_COUNT>(ix, nq, sm_count, &warps, &grid, &smem);
+    cudaError_t e = pairs_shape<RM, QUERY_COUNT, SW>(ix, nq, sm_count, &warps, &grid, &smem);
     if (e != cudaSuccess) return e;
     if (mode == QUERY_COUNT)
-        DSK_LAUNCH((lsh_pairs_kernel<QUERY_COUNT, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr,
+        DSK_LAUNCH((lsh_pairs_kernel<QUERY_COUNT, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr,
                    nullptr, nullptr, nullptr, removed, qsig, nq);
     else if (mode == QUERY_FILL)
-        DSK_LAUNCH((lsh_pairs_kernel<QUERY_FILL, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
+        DSK_LAUNCH((lsh_pairs_kernel<QUERY_FILL, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
                    nullptr, removed, qsig, nq);
     else
-        DSK_LAUNCH((lsh_pairs_kernel<QUERY_BEST, RM>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr, idx,
+        DSK_LAUNCH((lsh_pairs_kernel<QUERY_BEST, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr, idx,
                    eq, nullptr, removed, qsig, nq);
     return cudaGetLastError();
 }
 
 // The pair walk for the nq rows of qsig against the index's first n_docs documents.  counts != nullptr: counts[q] of the
 // kept candidates; ptr != nullptr: the fill of idx / eq at ptr[q]; else idx[q] / eq[q] = q's best kept candidate.
-cudaError_t launch_lsh_query_pairs(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count,
+cudaError_t launch_lsh_query_pairs(const LshDev &ix, int sw, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count,
                                    int64_t *counts, const int64_t *ptr, int32_t *idx, int32_t *eq, const uint32_t *removed,
                                    int sm_count, cudaStream_t s) {
     if (nq <= 0) return cudaSuccess;
     const int mode = counts ? QUERY_COUNT : ptr ? QUERY_FILL : QUERY_BEST;
-    if (removed) return launch_query_pairs_t<true>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, removed, sm_count, s);
-    return launch_query_pairs_t<false>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, nullptr, sm_count, s);
+    if (sw == 2) {
+        if (removed)
+            return launch_query_pairs_t<true, 2>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, removed, sm_count, s);
+        return launch_query_pairs_t<false, 2>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, nullptr, sm_count, s);
+    }
+    if (removed) return launch_query_pairs_t<true, 1>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, removed, sm_count, s);
+    return launch_query_pairs_t<false, 1>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, nullptr, sm_count, s);
 }
 
 }  // namespace dsk
@@ -989,25 +1013,25 @@ static unsigned unique_grid(int64_t work, int sm_count) {
 
 // Builds the batch table over sig (n rows), runs stage A against the first n_docs documents of ix, and writes counts[j] =
 // the number of row j's earlier partners in the batch.  No synchronisation.
-cudaError_t lsh_unique_count(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
-                             int64_t *counts, const uint32_t *removed, int sm_count, cudaStream_t s) {
+cudaError_t lsh_unique_count(const LshDev &ix, int sw, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count,
+                             void *ws, int64_t *counts, const uint32_t *removed, int sm_count, cudaStream_t s) {
     const UniqueWs w = unique_ws(ws, ix, sig, n, nullptr);
     cudaError_t e = cudaMemsetAsync(w.bt.slots, 0xFF, (size_t)ix.b * w.bt.cap_slots * 16, s);   // empty key, head -1
     if (e == cudaSuccess) e = launch_lsh_insert(w.bt, sig, 0, n, sm_count, s);
     if (e == cudaSuccess)
-        e = launch_lsh_query_pairs(ix, sig, n, n_docs, min_count, nullptr, nullptr, w.aidx, w.aeq, removed, sm_count, s);
-    if (e == cudaSuccess) e = launch_lsh_pairs(w.bt, n, min_count, counts, nullptr, nullptr, nullptr, nullptr, sm_count, s);
+        e = launch_lsh_query_pairs(ix, sw, sig, n, n_docs, min_count, nullptr, nullptr, w.aidx, w.aeq, removed, sm_count, s);
+    if (e == cudaSuccess) e = launch_lsh_pairs(w.bt, sw, n, min_count, counts, nullptr, nullptr, nullptr, nullptr, sm_count, s);
     return e;
 }
 
 // After lsh_unique_count and the scan of its counts into ptr: fills the batch pairs (pidx / peq), resolves the statuses,
 // writes kept / match / eq and new -> old, and returns *m = the number of kept rows.  Synchronises s once, to read m.
-cudaError_t lsh_unique_resolve(const LshDev &ix, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
+cudaError_t lsh_unique_resolve(const LshDev &ix, int sw, int64_t n_docs, const uint32_t *sig, int64_t n, int min_count, void *ws,
                                const int64_t *ptr, int32_t *pidx, int32_t *peq, uint8_t *kept, int32_t *match, int32_t *eq,
                                int64_t *m, int sm_count, cudaStream_t s) {
     const UniqueWs w = unique_ws(ws, ix, sig, n, nullptr);
     const unsigned grid = unique_grid(n, sm_count);
-    cudaError_t e = launch_lsh_pairs(w.bt, n, min_count, nullptr, ptr, pidx, peq, nullptr, sm_count, s);
+    cudaError_t e = launch_lsh_pairs(w.bt, sw, n, min_count, nullptr, ptr, pidx, peq, nullptr, sm_count, s);
     if (e != cudaSuccess) return e;
     DSK_LAUNCH(unique_init_kernel, grid, 256, 0, s, w.aidx, n, w.st);
     e = cudaMemsetAsync(w.list_n, 0, sizeof(unsigned), s);

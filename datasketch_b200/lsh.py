@@ -502,10 +502,18 @@ class GpuLSH:
     numbered in insertion order and ``keys`` (optional) maps numbers to user keys.  ``query``
     returns CSR arrays ``(ptr, idx)``: the candidates of query ``q`` are ``idx[ptr[q]:ptr[q+1]]``
     -- as a set, exactly ``MinHashLSH.query`` on the same data.
+
+    ``weighted=True`` indexes weighted MinHash signatures, as ``MinHashLSH(num_perm=ss)`` does with
+    ``WeightedMinHash`` objects: ``num_perm`` is the sample size ss, ``(b, r)`` count samples, and every method
+    that takes signatures takes ``[N, ss, 2]`` integer ``(k, t)`` rows (a numpy array, a CUDA tensor as
+    ``WeightedMinHashGenerator.minhash_batch(..., to_host=False)`` returns it, or a list of ``WeightedMinHash``)
+    with ``0 <= k < 2^32`` and ``-2^31 <= t < 2^31``.  Every ``eq`` then counts the samples whose ``(k, t)``
+    pairs agree, so ``eq / num_perm`` is ``WeightedMinHash.jaccard``, and the candidate sets are the reference's.
     """
 
     def __init__(self, threshold: float = 0.9, num_perm: int = 128, weights: Tuple[float, float] = (0.5, 0.5),
-                 params: Optional[Tuple[int, int]] = None, capacity: int = 1 << 20, device: int = 0):
+                 params: Optional[Tuple[int, int]] = None, capacity: int = 1 << 20, device: int = 0,
+                 weighted: bool = False):
         if params is not None:
             self.b, self.r = params
             if self.b * self.r > num_perm:
@@ -517,11 +525,13 @@ class GpuLSH:
         if self.b < 2:
             raise ValueError("The number of bands are too small (b < 2)")
         self.h = num_perm
+        self.weighted = bool(weighted)
         self.device = device
         self.capacity = int(capacity)
         nv.require_device(device)
         h = ctypes.c_void_p()
-        nv.check(nv.load().dsk_lsh_create(num_perm, self.b, self.r, self.capacity, device, ctypes.byref(h)))
+        create = nv.load().dsk_lsh_create_weighted if self.weighted else nv.load().dsk_lsh_create
+        nv.check(create(num_perm, self.b, self.r, self.capacity, device, ctypes.byref(h)))
         self._h = h
         self.keys: List[Hashable] = []
 
@@ -540,6 +550,8 @@ class GpuLSH:
 
     def _dev_sig(self, sig):
         import torch
+        if self.weighted:
+            return _pack_weighted(sig, self.h, torch.device("cuda", self.device))
         if isinstance(sig, np.ndarray):
             sig = torch.from_numpy(_signature_matrix(sig).view(np.int32)).cuda(self.device)
         if sig.dim() != 2 or sig.shape[1] != self.h:
@@ -563,8 +575,11 @@ class GpuLSH:
         """Append documents given as TOKEN lists (CUDA tensors: uint32/int32 or uint64/int64 hash values, int64 CSR
         offsets): ``MinHash.bulk`` + ``insert`` of every document (minhash.py:464-489, lsh.py:326-347) in one launch --
         the signature kernel builds each row straight into the index's storage and the warp that finishes a row does
-        its bucket updates (``dsk_lsh_insert_tokens``).  ``permutations`` is the (2, K) array of ``MinHash.permutations``."""
+        its bucket updates (``dsk_lsh_insert_tokens``).  ``permutations`` is the (2, K) array of ``MinHash.permutations``.
+        Not available on a weighted index (tokens give MinHash rows)."""
         import torch
+        if self.weighted:
+            raise ValueError("insert_tokens builds MinHash rows; a weighted index takes weighted MinHash signatures")
         if not d_tokens.is_cuda or not d_offsets.is_cuda or d_tokens.device.index != self.device \
                 or d_offsets.device.index != self.device:
             raise ValueError("insert_tokens needs CUDA tensors on device %d" % self.device)
@@ -622,7 +637,8 @@ class GpuLSH:
 
         ``idx[ptr[q]:ptr[q+1]]`` lists each candidate of query q once, in no particular order; without ``min_jaccard``
         the candidates, as a set, are ``query(sig)``'s.  ``eq`` is the number of the ``num_perm`` positions where the query
-        row and the document's row agree, so ``eq / num_perm`` is ``MinHash.jaccard``.  ``min_jaccard`` keeps only the
+        row and the document's row agree, so ``eq / num_perm`` is ``MinHash.jaccard`` (on a weighted index: the samples
+        whose ``(k, t)`` pairs agree, and ``WeightedMinHash.jaccard``).  ``min_jaccard`` keeps only the
         candidates with ``MinHash.jaccard >= min_jaccard``: ``[d for d in lsh.query(m) if m.jaccard(doc[d]) >= t]`` for
         every query at once, on the rows the index holds.  A query costs time linear in the size of the buckets it hits."""
         import torch
@@ -738,7 +754,8 @@ class GpuLSH:
 
         ``idx[ptr[i]:ptr[i+1]]`` holds (unordered) the documents ``d < i`` that ``query`` returns for document i's own row,
         and ``eq`` the number of the ``num_perm`` positions where the two rows agree, so ``eq / num_perm`` is
-        ``MinHash.jaccard`` of the pair.  ``min_jaccard`` keeps only the pairs with ``MinHash.jaccard >= min_jaccard``.
+        ``MinHash.jaccard`` of the pair (``WeightedMinHash.jaccard`` on a weighted index, where eq counts samples).
+        ``min_jaccard`` keeps only the pairs with ``MinHash.jaccard >= min_jaccard``.
         Runs on the device: one warp per document walks the document's buckets and compares the rows the index holds."""
         import torch
         mc = _jaccard_min_count(min_jaccard, self.h)
@@ -860,9 +877,51 @@ class GpuLSH:
         return remap.cpu().numpy() if to_host else remap
 
 
+_WMH_K_MAX = (1 << 32) - 1                      # k is packed as uint32
+_WMH_T_MIN, _WMH_T_MAX = -(1 << 31), (1 << 31) - 1   # t is packed as int32
+
+
+def _pack_weighted(sig, sample_size: int, device):
+    """Weighted MinHash rows -> the ``[N, 2 * sample_size]`` int32 tensor a weighted ``GpuLSH`` holds, on ``device``
+    (anything ``torch.device`` takes; the index passes its CUDA device).
+
+    ``sig`` is an ``[N, sample_size, 2]`` integer array of ``(k, t)`` pairs (numpy or a CUDA tensor) or a list of
+    ``WeightedMinHash``.  Sample j becomes word 2j = k_j as uint32 and word 2j + 1 = t_j as int32 (two's complement).  On
+    ``0 <= k < 2^32``, ``-2^31 <= t < 2^31`` the packing is injective, so equal words are equal pairs; values outside
+    raise ``ValueError`` naming the bound, before anything is sent to the index."""
+    import torch
+    dev = torch.device(device)
+    if isinstance(sig, torch.Tensor):
+        if sig.is_floating_point() or sig.is_complex() or sig.dtype in (torch.bool, torch.uint64):
+            raise TypeError("weighted MinHash rows must be a signed (or 8/16/32-bit unsigned) integer tensor")
+        x = sig.to(device=dev, dtype=torch.int64)   # exact for these types; the range is then checked on the device
+    else:
+        if not isinstance(sig, np.ndarray):
+            sig = list(sig)
+            sig = np.stack([np.asarray(m.hashvalues) for m in sig]) if sig else np.zeros((0, sample_size, 2), np.int64)
+        if sig.dtype.kind not in "iu":
+            raise TypeError("weighted MinHash rows must be integers")
+        x = sig
+    if x.ndim != 3 or x.shape[1] != sample_size or x.shape[2] != 2:
+        raise ValueError("Expecting weighted minhash rows of shape [N, %d, 2], got %s" % (sample_size, tuple(x.shape)))
+    k, t = x[..., 0], x[..., 1]
+    if x.shape[0]:
+        if bool((k < 0).any()) or bool((k > _WMH_K_MAX).any()):
+            raise ValueError("weighted MinHash k values must be in [0, 2^32 - 1]")
+        if bool((t < _WMH_T_MIN).any()) or bool((t > _WMH_T_MAX).any()):
+            raise ValueError("weighted MinHash t values must be in [-2^31, 2^31 - 1]")
+    if isinstance(x, np.ndarray):
+        x = torch.from_numpy(np.ascontiguousarray(x, dtype=np.int64))   # in range: exact
+    x = x.to(device=dev, dtype=torch.int64)
+    k, t = x[..., 0], x[..., 1]
+    k = k - ((k >> 31) << 32)                       # the uint32 bit pattern as an int32 value
+    return torch.stack([k, t], dim=-1).to(torch.int32).reshape(x.shape[0], 2 * sample_size).contiguous()
+
+
 def _jaccard_min_count(min_jaccard: Optional[float], num_perm: int) -> int:
     """The smallest count c in 0..num_perm with ``float(c) / float(num_perm) >= min_jaccard`` -- exactly the pairs
-    ``MinHash.jaccard(...) >= min_jaccard`` keeps (minhash.py:324 divides in float64 the same way).  None -> 0."""
+    ``MinHash.jaccard(...) >= min_jaccard`` keeps (minhash.py:324 divides in float64 the same way; so does
+    ``WeightedMinHash.jaccard``, weighted_minhash.py:60, with num_perm = the sample size).  None -> 0."""
     if min_jaccard is None:
         return 0
     t = float(min_jaccard)

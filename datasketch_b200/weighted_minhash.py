@@ -91,8 +91,9 @@ class WeightedMinHashGenerator:
         return st
 
     # -- sampling ----------------------------------------------------------------------------------
-    def _sample(self, X, device: int, many: bool, device_log: bool = False):
-        """Device pass over [n, dim] weights -> ([n, sample_size, 2] int64 of (k, t), [n] bool all-zero rows).
+    def _sample(self, X, device: int, many: bool, device_log: bool = False, to_host: bool = True):
+        """Device pass over [n, dim] weights -> ([n, sample_size, 2] int64 of (k, t), [n] bool all-zero rows), as numpy
+        arrays or (``to_host=False``) as the CUDA tensors the kernel wrote.
 
         For numpy input the logarithm is taken on the HOST with numpy's own float32 ``log`` -- the very call the
         reference makes (weighted_minhash.py:150-152: zeros -> NaN, ``vlog = np.log(v)``) -- and the kernel gets
@@ -125,13 +126,17 @@ class WeightedMinHashGenerator:
         with torch.cuda.device(device):
             nv.check(nv.load().dsk_wmh_minhash(h, d_v.data_ptr(), n, d_out.data_ptr(), d_st.data_ptr(), flags,
                                                torch.cuda.current_stream(d_v.device).cuda_stream))
+        if not to_host:
+            return d_out, d_st.bool()
         return d_out.cpu().numpy(), d_st.cpu().numpy().astype(bool)
 
-    def minhash_batch(self, X, device: int = 0, device_log: bool = False) -> np.ndarray:
+    def minhash_batch(self, X, device: int = 0, device_log: bool = False, to_host: bool = True):
         """[n, dim] weights -> [n, sample_size, 2] int64 of (k, t) -- row i equals
-        ``self.minhash(X[i]).hashvalues``.  Raises ValueError if any row is all zeros."""
-        out, empty = self._sample(X, device, many=False, device_log=device_log)
-        if empty.any():
+        ``self.minhash(X[i]).hashvalues``.  Raises ValueError if any row is all zeros.  ``to_host=False`` returns the
+        CUDA int64 tensor (the same values), which ``GpuLSH(weighted=True)`` takes as it is: weights -> signatures ->
+        index without a copy to the host."""
+        out, empty = self._sample(X, device, many=False, device_log=device_log, to_host=to_host)
+        if bool(empty.any()):
             raise ValueError("Input is all zeros")
         return out
 

@@ -252,6 +252,15 @@ DSK_API int dsk_wmh_minhash(const dsk_wmh *g, const float *d_v, int64_t n, int64
  *                        at most 64 MB for the rows.  It does not grow as n_docs * num_perm. */
 typedef struct dsk_lsh dsk_lsh;
 DSK_API int dsk_lsh_create(int num_perm, int b, int r, int64_t capacity_docs, int device, dsk_lsh **out);
+/* An index of WEIGHTED MinHash signatures (MinHashLSH over WeightedMinHash, lsh.py:344, weighted_minhash.py:55-60).  A row
+ * is [2 * sample_size] u32: sample j's (k_j, t_j) pair is word 2j = k_j as uint32 and word 2j + 1 = t_j as int32 (two's
+ * complement).  On 0 <= k < 2^32, -2^31 <= t < 2^31 this packing is injective, so two bands of r samples have equal
+ * reference keys (the byteswapped int64 pairs) iff their 2r words are equal, and band j of the reference is band j of a
+ * (b, 2r) banding over 2 * sample_size words.  b and r count samples (b * r <= sample_size).  Every entry below takes such
+ * rows in place of [n, num_perm] ones (dsk_lsh_insert, dsk_lsh_query_*, dsk_lsh_unique_*; the d_sig of dsk_lsh_unique_*
+ * must be 8-byte aligned), min_count is in [0, sample_size] and every eq counts SAMPLES whose two words both agree, so
+ * eq / sample_size is WeightedMinHash.jaccard.  dsk_lsh_insert_tokens returns DSK_ERR_INVALID for such an index. */
+DSK_API int dsk_lsh_create_weighted(int sample_size, int b, int r, int64_t capacity_docs, int device, dsk_lsh **out);
 DSK_API void dsk_lsh_destroy(dsk_lsh *ix);
 DSK_API int dsk_lsh_size(const dsk_lsh *ix, int64_t *n_docs, int64_t *capacity_docs);
 DSK_API int dsk_lsh_insert(dsk_lsh *ix, const uint32_t *d_sig, int64_t n, void *stream);
