@@ -65,6 +65,8 @@ SIGNATURES = {
     "dsk_lsh_query_jaccard_count": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
     "dsk_lsh_query_jaccard_fill": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "dsk_lsh_query_best": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    "dsk_lsh_query_topk": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "dsk_lsh_neighbors": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "dsk_lsh_unique_workspace_size": (ctypes.c_size_t, [c_void_p, c_int64]),
     "dsk_lsh_unique_count": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_size_t, c_void_p, c_void_p]),
     "dsk_lsh_unique_commit": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_size_t, c_void_p, c_void_p,

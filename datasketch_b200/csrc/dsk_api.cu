@@ -975,6 +975,46 @@ int dsk_lsh_query_best(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, in
     return run_query_pairs(ix, d_qsig, nq, min_count, nullptr, nullptr, d_idx, d_eq, stream);
 }
 
+static int check_topk(const char *who, int k) {
+    if (k < 1 || k > 32) {
+        set_error("%s: k must be in [1, 32] (got %d)", who, k);
+        return DSK_ERR_INVALID;
+    }
+    return DSK_OK;
+}
+
+// the first k kept candidates of nq query rows (qsig), or of every document's own row (qsig == nullptr, nq = n_docs)
+static int run_topk(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, int k, int32_t *d_idx,
+                    int32_t *d_eq, void *stream) {
+    if (nq == 0) return DSK_OK;
+    DevInfo *dev;
+    int rc = get_dev(ix->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(ix->device);
+    DSK_CUDA(launch_lsh_topk(ix->dev, ix->sw, d_qsig, nq, ix->n_docs, min_count, k, d_idx, d_eq, ix->walk_bitmap(),
+                             dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_lsh_query_topk(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, int k, int32_t *d_idx,
+                       int32_t *d_eq, void *stream) {
+    int rc = check_query_pairs("dsk_lsh_query_topk", ix, d_qsig, nq, min_count, d_idx && d_eq);
+    if (!rc) rc = check_topk("dsk_lsh_query_topk", k);
+    if (rc) return rc;
+    return run_topk(ix, d_qsig, nq, min_count, k, d_idx, d_eq, stream);
+}
+
+int dsk_lsh_neighbors(const dsk_lsh *ix, int min_count, int k, int32_t *d_idx, int32_t *d_eq, void *stream) {
+    int rc = check_self_join("dsk_lsh_neighbors", ix, min_count);
+    if (!rc) rc = check_topk("dsk_lsh_neighbors", k);
+    if (rc) return rc;
+    if (ix->n_docs > 0 && (!d_idx || !d_eq)) {
+        set_error("dsk_lsh_neighbors: null buffer");
+        return DSK_ERR_INVALID;
+    }
+    return run_topk(ix, nullptr, ix->n_docs, min_count, k, d_idx, d_eq, stream);
+}
+
 static int check_ids(const char *who, const dsk_lsh *ix, const void *d_docs, int64_t n, const void *d_out) {
     if (!ix) {
         set_error("%s: null handle", who);

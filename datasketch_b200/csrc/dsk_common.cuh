@@ -143,6 +143,11 @@ cudaError_t launch_lsh_clusters(const LshDev &ix, int sw, int64_t n_docs, int mi
 cudaError_t launch_lsh_query_pairs(const LshDev &ix, int sw, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count,
                                    int64_t *counts, const int64_t *ptr, int32_t *idx, int32_t *eq, const uint32_t *removed,
                                    int sm_count, cudaStream_t s);
+// each row's first k (1..32) kept candidates, larger eq first, then smaller d, -1 / -1 behind them, at idx / eq [row * k):
+// the nq rows of qsig against the first n_docs documents, or (qsig == nullptr) every document's own row against every
+// other document
+cudaError_t launch_lsh_topk(const LshDev &ix, int sw, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count, int k,
+                            int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s);
 // removal (bits of the bitmap) and compaction of the index
 cudaError_t launch_lsh_remove(uint32_t *removed, const int32_t *docs, int64_t n, int64_t n_docs, int64_t *status,
                               int sm_count, cudaStream_t s);

@@ -371,7 +371,8 @@ __global__ void __launch_bounds__(256) uf_flatten_kernel(int32_t *labels, int64_
     }
 }
 
-enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2, QUERY_COUNT = 3, QUERY_FILL = 4, QUERY_BEST = 5 };
+enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2, QUERY_COUNT = 3, QUERY_FILL = 4, QUERY_BEST = 5, QUERY_TOPK = 6,
+       SELF_TOPK = 7 };
 
 // warp <-> document i, lane <-> band (bands beyond 32 in further rounds), row i staged once in shared memory.  Each lane
 // probes its band's table with the fingerprint of i's own tuple and walks the bucket's chain to its next partner d: d < i,
@@ -389,7 +390,15 @@ enum { PAIRS_COUNT = 0, PAIRS_FILL = 1, PAIRS_UNION = 2, QUERY_COUNT = 3, QUERY_
 //   QUERY_FILL   written at idx / eq [ptr[i] ...), in no particular order
 //   QUERY_BEST   idx[i] / eq[i] = the kept partner with the largest eq, the smallest d among equal ones (-1 / -1: none).
 //                Each lane keeps its own best and a warp shuffle reduction picks the query's: no atomics.
-// In the PAIRS modes qsig and nq are unused and the code is the self-join's alone.
+// The TOPK modes keep the first `topk` (<= 32) kept partners in the order larger eq, then smaller d: lane j holds entry j,
+// -1 / -1 while empty.  Every candidate's eq is counted, and right after the count (where every lane knows the candidate and
+// its eq) a kept one is inserted at position popc(ballot(entry j is better)): the lanes above it shift up by one shuffle,
+// the lane at it takes the new entry, and a candidate that entry topk - 1 beats changes nothing.  At the end of the row
+// lanes < topk store idx / eq [i * topk + lane].  No shared-memory list and no atomics.
+//   QUERY_TOPK   the query walk (row i = qsig + i * k, every d < n_docs)
+//   SELF_TOPK    index row i against every document d < n_docs with d != i: i's nearest neighbours; with RM a removed i
+//                stores a row of -1 and skips its walk, warp-uniformly
+// In the PAIRS modes qsig and nq are unused and the code is the self-join's alone; only the TOPK modes read topk.
 // SW = words per sample.  SW = 1: MinHash rows, eq counts equal words.  SW = 2: weighted MinHash rows, sample s = words
 // 2s (k) and 2s + 1 (t), ix.k = 2 * sample_size and ix.r = 2 * r words; eq counts the samples whose two words are both
 // equal (WeightedMinHash.jaccard * sample_size), each read with one 8-byte load (rows of 2 * sample_size words stay 8-byte
@@ -399,22 +408,24 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
                                                         int64_t *__restrict__ counts, const int64_t *__restrict__ ptr,
                                                         int32_t *__restrict__ out_idx, int32_t *__restrict__ out_eq,
                                                         int32_t *labels, const uint32_t *__restrict__ removed,
-                                                        const uint32_t *__restrict__ qsig, int64_t nq) {
-    constexpr bool QUERY = MODE >= QUERY_COUNT;
+                                                        const uint32_t *__restrict__ qsig, int64_t nq, int topk) {
+    constexpr bool QUERY = MODE >= QUERY_COUNT && MODE != SELF_TOPK;
+    constexpr bool TOPK = MODE == QUERY_TOPK || MODE == SELF_TOPK;
     DSK_DYNAMIC_SMEM_T(uint32_t, s_rows, 16);   // [warps][k]
     const int lane = threadIdx.x & 31;
     uint32_t *row = s_rows + (int64_t)(threadIdx.x >> 5) * ix.k;
     const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
     const uint64_t mask = (uint64_t)ix.cap_slots - 1;
-    const bool need_eq = MODE == PAIRS_FILL || MODE == QUERY_FILL || MODE == QUERY_BEST || min_count > 0;
+    const bool need_eq = MODE == PAIRS_FILL || MODE == QUERY_FILL || MODE == QUERY_BEST || TOPK || min_count > 0;
     const unsigned below = (1u << lane) - 1u;
     for (int64_t i = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); i < (QUERY ? nq : n_docs); i += warps) {
         if (!QUERY && RM && is_removed(removed, i)) {
             if (MODE == PAIRS_COUNT && lane == 0) counts[i] = 0;
+            if (MODE == SELF_TOPK && lane < topk) { out_idx[i * topk + lane] = -1; out_eq[i * topk + lane] = -1; }
             continue;
         }
-        const int64_t bound = QUERY ? n_docs : i;   // partners d < bound
-        int32_t best_d = -1, best_eq = -1;          // QUERY_BEST: this lane's best kept partner
+        const int64_t bound = QUERY || MODE == SELF_TOPK ? n_docs : i;   // partners d < bound (SELF_TOPK: and d != i)
+        int32_t best_d = -1, best_eq = -1;          // QUERY_BEST: this lane's best kept partner; TOPK: entry `lane`
         const uint32_t *irow = (QUERY ? qsig : ix.sig) + i * ix.k;
         __syncwarp();
         for (int w = lane; w < ix.k; w += 32) row[w] = irow[w];
@@ -440,7 +451,7 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
                 while (d >= 0) {
                     const int32_t cur = d;
                     d = ix.next[(int64_t)cur * ix.b + band];
-                    if (cur < bound && !(RM && is_removed(removed, cur))) {
+                    if (cur < bound && !(MODE == SELF_TOPK && cur == i) && !(RM && is_removed(removed, cur))) {
                         const uint32_t *drow = ix.sig + (int64_t)cur * ix.k;
                         if (tuple_eq(drow + band * ix.r, it, ix.r)) {
                             bool dup = false;
@@ -469,6 +480,17 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
 #pragma unroll
                         for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xFFFFFFFFu, e, o);
                         if (lane == src) eq = e;
+                        if constexpr (TOPK) {   // e and c are the same in every lane: the insert is warp-uniform
+                            const int32_t c = __shfl_sync(0xFFFFFFFFu, cand, src);
+                            const bool better = lane < topk && (best_eq > e || (best_eq == e && best_d < c));
+                            const int at = __popc(__ballot_sync(0xFFFFFFFFu, better));   // entries before c
+                            if (e >= min_count && at < topk) {
+                                const int32_t ue = __shfl_up_sync(0xFFFFFFFFu, best_eq, 1);
+                                const int32_t ud = __shfl_up_sync(0xFFFFFFFFu, best_d, 1);
+                                if (lane == at) { best_eq = e; best_d = c; }
+                                else if (lane > at) { best_eq = ue; best_d = ud; }
+                            }
+                        }
                     }
                 }
                 const bool keep = cand >= 0 && eq >= min_count;
@@ -476,6 +498,8 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
                     if (keep) uf_union(labels, (int32_t)i, cand);
                 } else if (MODE == QUERY_BEST) {
                     if (keep && (eq > best_eq || (eq == best_eq && cand < best_d))) { best_eq = eq; best_d = cand; }
+                } else if (TOPK) {
+                    // inserted above, in the eq loop
                 } else {
                     const unsigned kept = __ballot_sync(0xFFFFFFFFu, keep);
                     if ((MODE == PAIRS_FILL || MODE == QUERY_FILL) && keep) {
@@ -496,6 +520,7 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
             }
             if (lane == 0) { out_idx[i] = best_d; out_eq[i] = best_eq; }
         }
+        if (TOPK && lane < topk) { out_idx[i * topk + lane] = best_d; out_eq[i * topk + lane] = best_eq; }
     }
 }
 
@@ -565,10 +590,10 @@ static cudaError_t launch_pairs_t(const LshDev &ix, int64_t n_docs, int min_coun
     if (e != cudaSuccess) return e;
     if (counts)
         DSK_LAUNCH((lsh_pairs_kernel<PAIRS_COUNT, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr,
-                   nullptr, nullptr, nullptr, removed, nullptr, 0);
+                   nullptr, nullptr, nullptr, removed, nullptr, 0, 0);
     else
         DSK_LAUNCH((lsh_pairs_kernel<PAIRS_FILL, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
-                   nullptr, removed, nullptr, 0);
+                   nullptr, removed, nullptr, 0, 0);
     return cudaGetLastError();
 }
 
@@ -602,7 +627,7 @@ static cudaError_t launch_clusters_t(const LshDev &ix, int64_t n_docs, int min_c
         cudaError_t e = pairs_shape<RM, PAIRS_COUNT, SW>(ix, n_docs, sm_count, &warps, &pg, &smem);
         if (e != cudaSuccess) return e;
         DSK_LAUNCH((lsh_pairs_kernel<PAIRS_UNION, RM, SW>), pg, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr,
-                   nullptr, nullptr, labels, removed, nullptr, 0);
+                   nullptr, nullptr, labels, removed, nullptr, 0, 0);
     }
     DSK_LAUNCH(uf_flatten_kernel<RM>, (unsigned)grid, 256, 0, s, labels, n_docs, removed);
     return cudaGetLastError();
@@ -630,13 +655,13 @@ static cudaError_t launch_query_pairs_t(const LshDev &ix, const uint32_t *qsig, 
     if (e != cudaSuccess) return e;
     if (mode == QUERY_COUNT)
         DSK_LAUNCH((lsh_pairs_kernel<QUERY_COUNT, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, counts, nullptr,
-                   nullptr, nullptr, nullptr, removed, qsig, nq);
+                   nullptr, nullptr, nullptr, removed, qsig, nq, 0);
     else if (mode == QUERY_FILL)
         DSK_LAUNCH((lsh_pairs_kernel<QUERY_FILL, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, ptr, idx, eq,
-                   nullptr, removed, qsig, nq);
+                   nullptr, removed, qsig, nq, 0);
     else
         DSK_LAUNCH((lsh_pairs_kernel<QUERY_BEST, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr, idx,
-                   eq, nullptr, removed, qsig, nq);
+                   eq, nullptr, removed, qsig, nq, 0);
     return cudaGetLastError();
 }
 
@@ -654,6 +679,38 @@ cudaError_t launch_lsh_query_pairs(const LshDev &ix, int sw, const uint32_t *qsi
     }
     if (removed) return launch_query_pairs_t<true, 1>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, removed, sm_count, s);
     return launch_query_pairs_t<false, 1>(ix, qsig, nq, n_docs, min_count, mode, counts, ptr, idx, eq, nullptr, sm_count, s);
+}
+
+template <bool RM, int SW>
+static cudaError_t launch_topk_t(const LshDev &ix, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count, int k,
+                                 int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s) {
+    const int64_t rows = qsig ? nq : n_docs;
+    int warps;
+    unsigned grid;
+    size_t smem;
+    cudaError_t e = pairs_shape<RM, QUERY_BEST, SW>(ix, rows, sm_count, &warps, &grid, &smem);   // QUERY_BEST, both TOPK
+    if (e != cudaSuccess) return e;
+    if (qsig)
+        DSK_LAUNCH((lsh_pairs_kernel<QUERY_TOPK, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr, idx,
+                   eq, nullptr, removed, qsig, nq, k);
+    else
+        DSK_LAUNCH((lsh_pairs_kernel<SELF_TOPK, RM, SW>), grid, 32 * warps, smem, s, ix, n_docs, min_count, nullptr, nullptr, idx,
+                   eq, nullptr, removed, nullptr, 0, k);
+    return cudaGetLastError();
+}
+
+// Each row's first k (1..32) kept partners, larger eq first, then smaller d, -1 / -1 behind them, at idx / eq [row * k ...):
+// qsig != nullptr: the nq query rows against the first n_docs documents; qsig == nullptr: the n_docs documents' own rows,
+// each against every other document (its nearest neighbours).
+cudaError_t launch_lsh_topk(const LshDev &ix, int sw, const uint32_t *qsig, int64_t nq, int64_t n_docs, int min_count, int k,
+                            int32_t *idx, int32_t *eq, const uint32_t *removed, int sm_count, cudaStream_t s) {
+    if ((qsig ? nq : n_docs) <= 0) return cudaSuccess;
+    if (sw == 2) {
+        if (removed) return launch_topk_t<true, 2>(ix, qsig, nq, n_docs, min_count, k, idx, eq, removed, sm_count, s);
+        return launch_topk_t<false, 2>(ix, qsig, nq, n_docs, min_count, k, idx, eq, nullptr, sm_count, s);
+    }
+    if (removed) return launch_topk_t<true, 1>(ix, qsig, nq, n_docs, min_count, k, idx, eq, removed, sm_count, s);
+    return launch_topk_t<false, 1>(ix, qsig, nq, n_docs, min_count, k, idx, eq, nullptr, sm_count, s);
 }
 
 }  // namespace dsk

@@ -683,6 +683,64 @@ class GpuLSH:
             return idx.cpu().numpy(), eq.cpu().numpy()
         return idx, eq
 
+    # -- the k most similar candidates, ranked on the device ---------------------------------------------------------------
+    def query_topk(self, sig, k: int, min_jaccard: Optional[float] = None, to_host: bool = True):
+        """Each query's k most similar indexed documents: ``(idx int32[Q, k], eq int32[Q, k])``.
+
+        Row q holds the first k candidates of ``query_jaccard(sig, min_jaccard)`` for query q in the order larger ``eq``
+        first, then smaller document number (a total order, so the result is fixed), best first; the slots behind them
+        are -1 / -1.  ``eq / num_perm`` is ``MinHash.jaccard`` (``WeightedMinHash.jaccard`` on a weighted index).  For a
+        query m this is::
+
+            sorted([d for d in lsh.query(m) if m.jaccard(doc[d]) >= t], key=lambda d: (-m.jaccard(doc[d]), d))[:k]
+
+        ``k`` is in ``[1, 32]``; ``query_topk(sig, 1)`` equals ``query_best(sig)``.  Removed documents are never listed.
+        One launch, without a host synchronisation, and an output of ``Q * k`` entries however many candidates a query
+        has; the walk and the verification cost what ``query_jaccard``'s do."""
+        import torch
+        k = _check_topk(k)
+        mc = _jaccard_min_count(min_jaccard, self.h)
+        d_q = self._dev_sig(sig)
+        nq = d_q.shape[0]
+        with torch.cuda.device(self.device):
+            idx = torch.empty((max(nq, 1), k), dtype=torch.int32, device=d_q.device)
+            eq = torch.empty((max(nq, 1), k), dtype=torch.int32, device=d_q.device)
+            nv.check(nv.load().dsk_lsh_query_topk(self._h, d_q.data_ptr(), nq, mc, k, idx.data_ptr(), eq.data_ptr(),
+                                                  torch.cuda.current_stream().cuda_stream))
+            idx, eq = idx[:nq], eq[:nq]
+        if to_host:
+            return idx.cpu().numpy(), eq.cpu().numpy()
+        return idx, eq
+
+    def neighbors(self, k: int, min_jaccard: Optional[float] = None, to_host: bool = True):
+        """The k nearest neighbours of every indexed document: ``(idx int32[n, k], eq int32[n, k])``, ``n = len(self)``.
+
+        Row i is ``query_topk``'s list for document i's own row with i itself left out: every other document d, below
+        or above i, that ``query`` returns for row i and that ``min_jaccard`` keeps, in the order larger ``eq`` first,
+        then smaller d, cut at k; -1 / -1 behind them.  For document i with row m this is::
+
+            sorted([d for d in lsh.query(m) if d != i and m.jaccard(doc[d]) >= t],
+                   key=lambda d: (-m.jaccard(doc[d]), d))[:k]
+
+        ``k`` is in ``[1, 32]``.  A removed document's row is all -1 and it appears in no list; after ``compact()`` rows
+        and numbers follow its ``remap``.  One launch, without a host synchronisation.  Each pair is verified from both
+        ends, about twice the row comparisons of ``candidate_pairs``: still quadratic in the size of each bucket; only
+        the output is bounded."""
+        import torch
+        k = _check_topk(k)
+        mc = _jaccard_min_count(min_jaccard, self.h)
+        n = len(self)
+        with torch.cuda.device(self.device):
+            dev = torch.device("cuda", self.device)
+            idx = torch.empty((max(n, 1), k), dtype=torch.int32, device=dev)
+            eq = torch.empty((max(n, 1), k), dtype=torch.int32, device=dev)
+            nv.check(nv.load().dsk_lsh_neighbors(self._h, mc, k, idx.data_ptr(), eq.data_ptr(),
+                                                 torch.cuda.current_stream().cuda_stream))
+            idx, eq = idx[:n], eq[:n]
+        if to_host:
+            return idx.cpu().numpy(), eq.cpu().numpy()
+        return idx, eq
+
     # -- streaming de-duplication: insert the rows that have no near-duplicate yet ---------------------------------------
     def insert_unique(self, sig, min_jaccard: Optional[float] = None, keys: Optional[Iterable[Hashable]] = None,
                       to_host: bool = True):
@@ -916,6 +974,13 @@ def _pack_weighted(sig, sample_size: int, device):
     k, t = x[..., 0], x[..., 1]
     k = k - ((k >> 31) << 32)                       # the uint32 bit pattern as an int32 value
     return torch.stack([k, t], dim=-1).to(torch.int32).reshape(x.shape[0], 2 * sample_size).contiguous()
+
+
+def _check_topk(k) -> int:
+    """``k`` of ``query_topk`` / ``neighbors``: an integer in [1, 32] (the entries one warp holds), else ``ValueError``."""
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= 32:
+        raise ValueError("k must be an integer in [1, 32], got %r" % (k,))
+    return int(k)
 
 
 def _jaccard_min_count(min_jaccard: Optional[float], num_perm: int) -> int:

@@ -293,6 +293,21 @@ DSK_API int dsk_lsh_query_jaccard_fill(const dsk_lsh *ix, const uint32_t *d_qsig
                                        const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq, void *stream);
 DSK_API int dsk_lsh_query_best(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, int32_t *d_idx,
                                int32_t *d_eq, void *stream);
+/* The k most similar kept candidates of each row, ranked on the device (the candidates of dsk_lsh_query_jaccard_fill, sorted
+ * by eq descending, then document number ascending, and cut at k).  k in [1, 32]; min_count as above.  Row q's list is at
+ * d_idx[q * k .. q * k + k) with its eq at the same positions of d_eq, best first; the slots behind the last kept candidate
+ * hold -1 / -1.  Removed documents (since the last dsk_lsh_compact) are never listed.  One launch: no count, scan or fill,
+ * no workspace, no synchronisation.  The walk and the verification are dsk_lsh_query_jaccard_count's; only the output is
+ * bounded (k entries per row).
+ *   dsk_lsh_query_topk   d_qsig [nq, num_perm] u32 query rows, d_idx / d_eq [nq, k].  k = 1 gives dsk_lsh_query_best.
+ *                        nq == 0 with null buffers is a valid no-op.
+ *   dsk_lsh_neighbors    every document i's own row against every other document d != i (d < i and d > i): i's k nearest
+ *                        neighbours, d_idx / d_eq [n_docs, k].  A removed document's row is all -1.  Each pair is verified
+ *                        from both ends, about twice dsk_lsh_pairs_count's row comparisons.  An empty index with null
+ *                        buffers is a valid no-op. */
+DSK_API int dsk_lsh_query_topk(const dsk_lsh *ix, const uint32_t *d_qsig, int64_t nq, int min_count, int k, int32_t *d_idx,
+                               int32_t *d_eq, void *stream);
+DSK_API int dsk_lsh_neighbors(const dsk_lsh *ix, int min_count, int k, int32_t *d_idx, int32_t *d_eq, void *stream);
 /* Streaming de-duplication of a batch (the loop `for m in batch: if not [d for d in lsh.query(m) if m.jaccard(doc[d]) >= t]:
  * lsh.insert(key, m)`, lsh.py:326-347 / :370-432, minhash.py:299-324), on the device.  Row j of d_sig ([n, num_perm] u32)
  * is KEPT iff no remaining (not removed) document of the index and no row j' < j of the batch that was kept is a candidate

@@ -33,11 +33,12 @@ def ev_time(fn, iters=3, warm=1):
 
 
 def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, remove_leg=False, query_jaccard_leg=False,
-       insert_unique_leg=False, n_unique=100_000):
+       insert_unique_leg=False, n_unique=100_000, topk_leg=False):
     """10M x 128 tokens, K=256 + LSH(0.8) insert + query (here n_docs on one GPU).  dedup_leg: also the self-join of
     the index (candidate_pairs, duplicate_clusters with and without min_jaccard=0.8) against the host flow it replaces.
     remove_leg: also removal of the duplicates from the index and its compaction (c3_remove).  query_jaccard_leg: also
-    queries verified on the device against the two-step flow they replace (c3_query_jaccard).  insert_unique_leg: also
+    queries verified on the device against the two-step flow they replace (c3_query_jaccard).  topk_leg: also the ranked
+    lists query_topk / neighbors against the flows they replace (c3_topk).  insert_unique_leg: also
     GpuLSH.insert_unique of a batch of n_unique fresh documents against the flow it replaces (c3_insert_unique); the index
     then has room for them (its bucket tables are the same size)."""
     perms = _make_permutations(k, 1)
@@ -109,6 +110,8 @@ def c3(n_docs, t=128, k=256, n_query=100_000, fused_leg=False, dedup_leg=False, 
         dedup.update(c3_remove(lsh, sig, q))
     if query_jaccard_leg:
         dedup.update(c3_query_jaccard(lsh, sig, tok, perms))
+    if topk_leg:
+        dedup.update(c3_topk(lsh, tok, perms))
     if insert_unique_leg:
         dedup.update(c3_insert_unique(lsh, tok, perms, n_unique))
     return {"config": "C3 (1 GPU)", "docs": n_docs, "tokens": t, "num_perm": k, "b": lsh.b, "r": lsh.r,
@@ -227,13 +230,9 @@ def gpu_card():
     return {"gpu": name, "power_limit_w": float(watts), "sm_clock_max_mhz": float(mhz)}
 
 
-def c3_query_jaccard(lsh, sig, tok, perms, n_query=100_000, min_jaccard=0.8, rounds=3):
-    """GpuLSH.query_jaccard / query_best for n_query fresh documents against the C3 index: half of them copies of indexed
-    documents with 10 % of the tokens resampled, half unrelated, their signatures built by the same kernel.  Beside them,
-    query() and the two-step flow they replace: query, the (query, document) pairs expanded with repeat_interleave,
-    codec.jaccard_pairs on cat([index rows, queries]) and the filter re-packed as CSR.  Each round times every call with
-    CUDA events (3 calls after 1 warm-up call), the calls alternating; the outputs are compared in the same run."""
-    n, k = len(lsh), lsh.h
+def c3_fresh_queries(n, tok, perms, n_query):
+    """Signatures of n_query fresh documents against the first n rows of `tok`: half of them copies of indexed documents
+    with 10 % of the tokens resampled, half unrelated, built by the same signature kernel (the same rows on every call)."""
     t = tok.shape[1]
     g = torch.Generator(device="cuda").manual_seed(11)
     qtok = torch.randint(-2 ** 31, 2 ** 31 - 1, (n_query, t), dtype=torch.int32, device="cuda", generator=g)
@@ -241,7 +240,17 @@ def c3_query_jaccard(lsh, sig, tok, perms, n_query=100_000, min_jaccard=0.8, rou
     src = torch.randint(0, n, (h,), device="cuda", generator=g)
     qtok[:h] = torch.where(torch.rand((h, t), device="cuda", generator=g) < 0.1, qtok[:h], tok[src])
     qoff = torch.arange(0, (n_query + 1) * t, t, dtype=torch.int64, device="cuda")
-    qs = dsk.engine.bulk_signatures_device(qtok.view(-1), qoff, n_query * t, perms)
+    return dsk.engine.bulk_signatures_device(qtok.view(-1), qoff, n_query * t, perms)
+
+
+def c3_query_jaccard(lsh, sig, tok, perms, n_query=100_000, min_jaccard=0.8, rounds=3):
+    """GpuLSH.query_jaccard / query_best for n_query fresh documents against the C3 index: half of them copies of indexed
+    documents with 10 % of the tokens resampled, half unrelated, their signatures built by the same kernel.  Beside them,
+    query() and the two-step flow they replace: query, the (query, document) pairs expanded with repeat_interleave,
+    codec.jaccard_pairs on cat([index rows, queries]) and the filter re-packed as CSR.  Each round times every call with
+    CUDA events (3 calls after 1 warm-up call), the calls alternating; the outputs are compared in the same run."""
+    n, k = len(lsh), lsh.h
+    qs = c3_fresh_queries(n, tok, perms, n_query)
     ar = torch.arange(n_query, device="cuda")
 
     def two_step(thr):
@@ -289,6 +298,72 @@ def c3_query_jaccard(lsh, sig, tok, perms, n_query=100_000, min_jaccard=0.8, rou
     for name, ts in times.items():
         out["qj_%s_ms" % name] = ts
     out.update({"qj_" + key: v for key, v in gpu_card().items()})
+    return out
+
+
+def segmented_topk(rows, idx, eq, n_rows, n_idx, k, num_perm):
+    """(row, idx, eq) triples on the device -> ``[n_rows, k]`` idx / eq, per row sorted by larger eq, then smaller idx, cut
+    at k and padded with -1: one torch sort of a combined int64 key (row, num_perm - eq, idx), then the rank in the row."""
+    key = (rows.long() * (num_perm + 1) + (num_perm - eq.long())) * n_idx + idx.long()
+    key, order = torch.sort(key)
+    rows, idx, eq = rows[order].long(), idx[order], eq[order]
+    start = torch.searchsorted(rows, torch.arange(n_rows, device=rows.device))
+    rank = torch.arange(len(rows), device=rows.device) - start[rows]
+    sel = rank < k
+    oi = torch.full((n_rows, k), -1, dtype=torch.int32, device=rows.device)
+    oe = torch.full((n_rows, k), -1, dtype=torch.int32, device=rows.device)
+    oi[rows[sel], rank[sel]] = idx[sel].int()
+    oe[rows[sel], rank[sel]] = eq[sel].int()
+    return oi, oe
+
+
+def c3_topk(lsh, tok, perms, n_query=100_000, k=10, min_jaccard=0.5, best_jaccard=0.8, rounds=3):
+    """GpuLSH.query_topk / neighbors on the C3 index, each beside the flow it replaces: query_topk(k, min_jaccard) of
+    n_query fresh documents (built as in c3_query_jaccard) against query_jaccard(min_jaccard) + a torch segmented top-k,
+    query_topk(1, best_jaccard) against query_best(best_jaccard), and neighbors(k, min_jaccard) against
+    candidate_pairs(min_jaccard) made symmetric + the same top-k.  Each round times every call with CUDA events (3 calls
+    after 1 warm-up call), the calls alternating; the outputs are compared in the same run."""
+    n, K = len(lsh), lsh.h
+    qs = c3_fresh_queries(n, tok, perms, n_query)
+    ar_q, ar_n = torch.arange(n_query, device="cuda"), torch.arange(n, device="cuda")
+
+    def query_flow():
+        p, x, e = lsh.query_jaccard(qs, min_jaccard, to_host=False)
+        return segmented_topk(torch.repeat_interleave(ar_q, p[1:] - p[:-1]), x, e, n_query, n, k, K)
+
+    def neighbors_flow():
+        p, x, e = lsh.candidate_pairs(min_jaccard, to_host=False)
+        i = torch.repeat_interleave(ar_n, p[1:] - p[:-1])
+        return segmented_topk(torch.cat([i, x.long()]), torch.cat([x, i.int()]), torch.cat([e, e]), n, n, k, K)
+
+    calls = {"query_topk": lambda: lsh.query_topk(qs, k, min_jaccard, to_host=False),
+             "query_jaccard_torch_topk": query_flow,
+             "query_topk_1": lambda: lsh.query_topk(qs, 1, best_jaccard, to_host=False),
+             "query_best": lambda: lsh.query_best(qs, best_jaccard, to_host=False),
+             "neighbors": lambda: lsh.neighbors(k, min_jaccard, to_host=False),
+             "candidate_pairs_symmetric_torch_topk": neighbors_flow}
+    times = {name: [] for name in calls}
+    for _ in range(rounds):
+        for name, fn in calls.items():
+            times[name].append(ev_time(fn))
+    qi, qe = lsh.query_topk(qs, k, min_jaccard, to_host=False)
+    fi, fe = query_flow()
+    ti, te = lsh.query_topk(qs, 1, best_jaccard, to_host=False)
+    bi, be = lsh.query_best(qs, best_jaccard, to_host=False)
+    ni, ne = lsh.neighbors(k, min_jaccard, to_host=False)
+    si, se = neighbors_flow()
+    p, _, _ = lsh.query_jaccard(qs, min_jaccard, to_host=False)
+    pp, _, _ = lsh.candidate_pairs(min_jaccard, to_host=False)
+    out = {"tk_queries": n_query, "tk_k": k, "tk_min_jaccard": min_jaccard, "tk_best_min_jaccard": best_jaccard,
+           "tk_query_candidates_kept": int(p[-1].item()), "tk_queries_with_a_match": int((qi[:, 0] >= 0).sum().item()),
+           "tk_query_entries": int((qi >= 0).sum().item()), "tk_pairs_kept": int(pp[-1].item()),
+           "tk_docs_with_a_neighbor": int((ni[:, 0] >= 0).sum().item()), "tk_neighbor_entries": int((ni >= 0).sum().item()),
+           "tk_query_topk_equals_flow": bool(torch.equal(qi, fi) and torch.equal(qe, fe)),
+           "tk_query_topk_1_equals_query_best": bool(torch.equal(ti[:, 0], bi) and torch.equal(te[:, 0], be)),
+           "tk_neighbors_equals_flow": bool(torch.equal(ni, si) and torch.equal(ne, se))}
+    for name, ts in times.items():
+        out["tk_%s_ms" % name] = ts
+    out.update({"tk_" + key: v for key, v in gpu_card().items()})
     return out
 
 
@@ -478,10 +553,15 @@ if __name__ == "__main__":
                     help="also time GpuLSH.insert_unique(0.8) of 100k fresh documents against the C3 index, beside the "
                          "flow it replaces (query_best, a temporary index's candidate_pairs, a host greedy loop, insert), "
                          "and compare their outputs")
+    ap.add_argument("--c3-topk", action="store_true",
+                    help="also time GpuLSH.query_topk(10, 0.5) / query_topk(1, 0.8) for 100k fresh documents and "
+                         "neighbors(10, 0.5) on the C3 index, beside the flows they replace (query_jaccard + a torch "
+                         "segmented top-k, query_best, symmetrised candidate_pairs + the same top-k), and compare outputs")
     a = ap.parse_args()
     if a.c3_docs > 0:
         print(json.dumps(c3(a.c3_docs, fused_leg=a.c3_fused, dedup_leg=a.c3_dedup, remove_leg=a.c3_remove,
-                            query_jaccard_leg=a.c3_query_jaccard, insert_unique_leg=a.c3_insert_unique)), flush=True)
+                            query_jaccard_leg=a.c3_query_jaccard, insert_unique_leg=a.c3_insert_unique,
+                            topk_leg=a.c3_topk)), flush=True)
     for fn, arg in ((c4, a.c4_vecs), (c5, a.c5_rows)):
         if arg > 0:
             print(json.dumps(fn(arg)), flush=True)
