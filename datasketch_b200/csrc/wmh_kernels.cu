@@ -2,19 +2,25 @@
 //
 // Replaces the per-sample Python loop of WeightedMinHashGenerator.minhash
 // (datasketch/weighted_minhash.py:147-158) for batches of vectors:
-//   vlog = log(v)                      (zeros -> NaN and are skipped, :148-152)
+//   vlog = log(v)                      (zeros -> -inf and are skipped in both modes)
 //   t    = floor(vlog / r_i + beta_i)
 //   ln_y = (t - beta_i) * r_i
 //   ln_a = (ln_c_i - ln_y) - r_i
-//   k    = first index of the NaN-skipping minimum of ln_a;  out[i] = (k, int(t[k]))
+//   k    = first index of the NaN-skipping minimum of ln_a (np.nanargmin);  out[i] = (k, int(t[k]))
 // MANY = true evaluates the reference's experimental minhash_many instead (weighted_minhash.py:221-224):
 //   ln_y = ((t - beta_i) + 1) * r_i;  ln_a = ln_c_i - ln_y      (same algebra, different float32 rounding)
-// and an all-zero row is reported in status[] (the caller returns None for it, :228 / :241-245).
+// and takes np.argmin over the row's non-zero columns: a NaN ln_a (negative or NaN weight) wins at its first occurrence.
+// A row with no candidate column (all zeros; in minhash mode also all negative / NaN) is reported in status[] (the
+// caller raises ValueError or returns None for it, :149-150 / :241-245).  A +inf weight gives ln_a = -inf, which wins
+// every sample with t = +inf; a non-finite t is stored as INT64_MIN (numpy's float -> int64 cast on x86-64) and the row
+// is reported as status 2 (the reference's int(t) raises OverflowError in minhash).
 // Every float32 operation is a separate IEEE round-to-nearest op in exactly that order
 // (__fdiv_rn/__fadd_rn/__fsub_rn/__fmul_rn: no FMA contraction, no fast-math), so all steps after
-// the logarithm are bit-identical to numpy; the logarithm is log() in double rounded to float32
-// (numpy's SIMD float32 log is not correctly rounded, so this one step agrees to <= 1 ulp; see
-// DESIGN.md and tests/test_wmh_gpu.py for the measured effect on (k, t): none on the fixtures).
+// the logarithm are bit-identical to numpy.  The device's own logarithm is log() in double rounded to float32, i.e. the
+// correctly rounded float32 log unless the double lies within a few double ulps of a float32 rounding midpoint.  numpy's
+// SIMD float32 log is not correctly rounded (up to 3 ulp off on x86-64 hosts), so the host layer passes numpy's vlog
+// (DSK_WMH_INPUT_LOG) where the reference's exact values matter; tests/test_wmh_edges_gpu.py checks the device-log
+// results exactly against the float64 log rounded to float32, and against numpy's log up to float64-confirmed near-ties.
 //
 // Layout: parameters are stored transposed, [dim][ss_pad], so the threads of a CTA (one per
 // sample) read consecutive addresses; they are 3 * ss * dim * 4 B (6.3 MB at dim 4096, ss 128) and
@@ -33,8 +39,8 @@ struct WmhParams {
     const float *v;                        // [n][dim]
     int64_t n;
     int64_t *out;                          // [n][ss][2]
-    int32_t *status;                       // [n]: 1 = all-zero input (weighted_minhash.py:149-150)
-    int input_log;                         // v already holds ln(weight) as float32 (NaN where the weight is zero)
+    int32_t *status;                       // [n]: 0, 1 = no candidate column, 2 = the winning t is not finite
+    int input_log;                         // v already holds ln(weight) as float32 (-inf where the weight is zero)
 };
 
 // ln_a for one (sample, dim): each float32 operation rounded separately, in the reference's order
@@ -47,6 +53,14 @@ __device__ __forceinline__ float wmh_ln_a(float t, float be, float r, float lc) 
         const float ln_y = __fmul_rn(__fsub_rn(t, be), r);
         return __fsub_rn(__fsub_rn(lc, ln_y), r);
     }
+}
+
+// Does ln_a replace the running minimum?  Strict, so the first index wins ties in both modes.  A zero weight
+// (vlog = -inf) gives ln_a = +inf, which never does; every other finite or +inf vlog gives a finite or -inf ln_a.
+template <bool MANY>
+__device__ __forceinline__ bool wmh_better(float ln_a, float best) {
+    if constexpr (MANY) return ln_a < best || (ln_a != ln_a && best == best);  // np.argmin: the first NaN wins
+    else return ln_a < best;                                                     // np.nanargmin: NaN never wins
 }
 
 template <bool MANY>
@@ -69,13 +83,12 @@ __global__ void __launch_bounds__(kWmhThreads) wmh_kernel(const WmhParams p) {
             __syncthreads();  // previous tile fully consumed
             for (int idx = tid; idx < kVec * kTileD; idx += kWmhThreads) {
                 const int u = idx / kTileD, dd = idx - u * kTileD;
-                float lg = __int_as_float(0x7fc00000);  // NaN: padding and zero weights are skipped
+                float lg = __int_as_float(0xff800000);  // -inf: padding is skipped like a zero weight
                 if (dd < nd && u0 + u < p.n) {
                     const float x = __ldg(p.v + (u0 + u) * (int64_t)p.dim + d0 + dd);
                     // host-computed logarithms (numpy's own float32 log: bit-identical to the reference by
-                    // construction) or, opt-in, the device's correctly rounded one (<= 1 ulp from numpy's)
-                    if (p.input_log) lg = x;
-                    else if (x != 0.f) lg = (float)log((double)x);
+                    // construction) or the device's: log(+-0) = -inf, log(x < 0) = NaN, log(+inf) = +inf
+                    lg = p.input_log ? x : (float)log((double)x);
                 }
                 s_vlog[dd][u] = lg;
             }
@@ -105,7 +118,7 @@ __global__ void __launch_bounds__(kWmhThreads) wmh_kernel(const WmhParams p) {
                         for (int u = 0; u < kVec; ++u) {
                             const float t = floorf(__fadd_rn(__fdiv_rn(xs[u], r[q]), be[q]));
                             const float ln_a = wmh_ln_a<MANY>(t, be[q], r[q], lc[q]);
-                            if (ln_a < best[u] || (bk[u] < 0 && ln_a == ln_a)) {  // NaN never wins; first index kept on ties
+                            if (wmh_better<MANY>(ln_a, best[u])) {
                                 best[u] = ln_a; bk[u] = d0 + dd + q; bt[u] = t;
                             }
                         }
@@ -122,7 +135,7 @@ __global__ void __launch_bounds__(kWmhThreads) wmh_kernel(const WmhParams p) {
                     for (int u = 0; u < kVec; ++u) {
                         const float t = floorf(__fadd_rn(__fdiv_rn(xs[u], r), be));
                         const float ln_a = wmh_ln_a<MANY>(t, be, r, lc);
-                        if (ln_a < best[u] || (bk[u] < 0 && ln_a == ln_a)) {
+                        if (wmh_better<MANY>(ln_a, best[u])) {
                             best[u] = ln_a; bk[u] = d0 + dd; bt[u] = t;
                         }
                     }
@@ -134,9 +147,12 @@ __global__ void __launch_bounds__(kWmhThreads) wmh_kernel(const WmhParams p) {
             for (int u = 0; u < kVec; ++u) {
                 if (u0 + u < p.n) {
                     int64_t *o = p.out + ((u0 + u) * (int64_t)p.ss + s) * 2;
+                    const bool fin = isfinite(bt[u]);
                     o[0] = bk[u] < 0 ? 0 : bk[u];
-                    o[1] = bk[u] < 0 ? 0 : (int64_t)bt[u];
-                    if (s == 0) p.status[u0 + u] = bk[u] < 0 ? 1 : 0;
+                    o[1] = bk[u] < 0 ? 0 : fin ? (int64_t)bt[u] : INT64_MIN;
+                    // t is non-finite in one sample exactly when the row holds a +inf weight (or, in MANY mode, a
+                    // NaN ln_a), and then in every sample, so sample 0 speaks for the row
+                    if (s == 0) p.status[u0 + u] = bk[u] < 0 ? 1 : fin ? 0 : 2;
                 }
             }
         }

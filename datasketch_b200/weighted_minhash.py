@@ -92,14 +92,18 @@ class WeightedMinHashGenerator:
 
     # -- sampling ----------------------------------------------------------------------------------
     def _sample(self, X, device: int, many: bool, device_log: bool = False, to_host: bool = True):
-        """Device pass over [n, dim] weights -> ([n, sample_size, 2] int64 of (k, t), [n] bool all-zero rows), as numpy
-        arrays or (``to_host=False``) as the CUDA tensors the kernel wrote.
+        """Device pass over [n, dim] weights -> ([n, sample_size, 2] int64 of (k, t), [n] int32 status), as numpy
+        arrays or (``to_host=False``) as the CUDA tensors the kernel wrote.  Status 1 marks a row with no candidate
+        column (all zeros; for ``many=False`` also all negative or NaN), status 2 a row whose t is not finite (a +inf
+        weight; stored as INT64_MIN).
 
         For numpy input the logarithm is taken on the HOST with numpy's own float32 ``log`` -- the very call the
-        reference makes (weighted_minhash.py:150-152: zeros -> NaN, ``vlog = np.log(v)``) -- and the kernel gets
-        ``vlog`` (``DSK_WMH_INPUT_LOG``), so every step is bit-identical to the reference by construction.
-        ``device_log=True`` (and CUDA tensor input) lets the kernel take the logarithm itself: one pass less over
-        the data, values within 1 ulp of numpy's, the same (k, t) except on float near-ties."""
+        reference makes (weighted_minhash.py:150-152, ``vlog = np.log(v)``; zeros give -inf here and are skipped) --
+        and the kernel gets ``vlog`` (``DSK_WMH_INPUT_LOG``), so every step is bit-identical to the reference by
+        construction.  ``device_log=True`` (and CUDA tensor input) lets the kernel take the logarithm itself: one
+        pass less over the data.  Its log is the float64 log rounded to float32, which is not always numpy's (numpy's
+        float32 log can be up to 3 ulp from the correctly rounded one), so (k, t) can differ from the reference's on
+        float near-ties."""
         import torch
         flags = int(many)
         if isinstance(X, np.ndarray):
@@ -108,8 +112,6 @@ class WeightedMinHashGenerator:
                 raise ValueError("Input dimension mismatch, expecting %d" % self.dim)
             h = self._handle(device)
             if not device_log:
-                X = X.copy()
-                X[X == 0] = np.nan
                 with np.errstate(invalid="ignore", divide="ignore"):
                     X = np.log(X)
                 flags |= 2   # DSK_WMH_INPUT_LOG
@@ -127,21 +129,29 @@ class WeightedMinHashGenerator:
             nv.check(nv.load().dsk_wmh_minhash(h, d_v.data_ptr(), n, d_out.data_ptr(), d_st.data_ptr(), flags,
                                                torch.cuda.current_stream(d_v.device).cuda_stream))
         if not to_host:
-            return d_out, d_st.bool()
-        return d_out.cpu().numpy(), d_st.cpu().numpy().astype(bool)
+            return d_out, d_st
+        return d_out.cpu().numpy(), d_st.cpu().numpy()
+
+    @staticmethod
+    def _raise_status(status, empty_message: str) -> None:
+        worst = int(status.max()) if len(status) else 0
+        if worst and bool((status == 1).any()):
+            raise ValueError(empty_message)
+        if worst:
+            raise OverflowError("cannot convert float infinity to integer")   # the reference's int(t[k]) (:158)
 
     def minhash_batch(self, X, device: int = 0, device_log: bool = False, to_host: bool = True):
         """[n, dim] weights -> [n, sample_size, 2] int64 of (k, t) -- row i equals
-        ``self.minhash(X[i]).hashvalues``.  Raises ValueError if any row is all zeros.  ``to_host=False`` returns the
-        CUDA int64 tensor (the same values), which ``GpuLSH(weighted=True)`` takes as it is: weights -> signatures ->
-        index without a copy to the host."""
-        out, empty = self._sample(X, device, many=False, device_log=device_log, to_host=to_host)
-        if bool(empty.any()):
-            raise ValueError("Input is all zeros")
+        ``self.minhash(X[i]).hashvalues``.  Raises ValueError if a row has no positive weight and OverflowError if
+        one holds +inf.  ``to_host=False`` returns the CUDA int64 tensor (the same values), which
+        ``GpuLSH(weighted=True)`` takes as it is: weights -> signatures -> index without a copy to the host."""
+        out, status = self._sample(X, device, many=False, device_log=device_log, to_host=to_host)
+        self._raise_status(status, "Input is all zeros")
         return out
 
     def minhash(self, v) -> WeightedMinHash:
-        """One weighted Jaccard vector -> WeightedMinHash (weighted_minhash.py:123-159; same checks)."""
+        """One weighted Jaccard vector -> WeightedMinHash (weighted_minhash.py:123-159; same checks and errors:
+        ValueError for an all-zero vector or one without a positive weight, OverflowError for a +inf weight)."""
         if not isinstance(v, collections.abc.Sized):
             raise TypeError("Input vector must be sized")
         if not len(v) == self.dim:
@@ -149,12 +159,15 @@ class WeightedMinHashGenerator:
         v = np.array(v, dtype=np.float32)  # a private float32 copy: the input is never mutated
         if not (v != 0).any():
             raise ValueError("Input is all zeros")
-        out = self.minhash_batch(v.reshape(1, -1))
+        out, status = self._sample(v.reshape(1, -1), 0, many=False)
+        self._raise_status(status, "All-NaN slice encountered")   # np.nanargmin's error (:157)
         return WeightedMinHash(self.seed, out[0].astype(int, copy=False))
 
     def minhash_many(self, X, device: int = 0) -> List[Optional[WeightedMinHash]]:
         """A matrix of weighted Jaccard vectors (rows; numpy or scipy.sparse) -> one WeightedMinHash per
         row, ``None`` for an all-zero row (weighted_minhash.py:161-247; same checks and return type).
+        As there, the first negative or NaN weight of a row wins every sample, and a non-finite t (that one, or a
+        +inf weight) is stored as INT64_MIN.
 
         The reference's experimental method rounds ``ln_a`` in a different order than ``minhash``
         (:221-224: ``ln_y = (t - beta + 1) * r; ln_a = ln_c - ln_y``); the kernel's
@@ -176,8 +189,8 @@ class WeightedMinHashGenerator:
         for r0 in range(0, n, slab):
             part = X[r0:r0 + slab]
             dense = np.asarray(part.toarray() if sparse else part, dtype=np.float32)
-            out, empty = self._sample(dense, device, many=True)
+            out, status = self._sample(dense, device, many=True)
             for i in range(out.shape[0]):
-                if not empty[i]:
+                if status[i] != 1:
                     ret[r0 + i] = WeightedMinHash(self.seed, out[i].astype(int, copy=False))
         return ret

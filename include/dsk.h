@@ -189,13 +189,19 @@ DSK_API int dsk_bloom_query(const uint32_t *d_sig, int64_t n, int num_perm, int 
  * (datasketch/weighted_minhash.py:118-121).  dsk_wmh_minhash replaces the per-sample loop
  * of WeightedMinHashGenerator.minhash (:147-158) for a batch of n vectors:
  *   d_v      [n, dim] float32 weights (zeros are skipped, :148-152)
- *   d_out    [n, sample_size, 2] int64: (k, int(t_k)) per sample (:158)
- *   d_status [n] int32: 1 where the input row is all zeros (reference: ValueError, :149-150)
- *   flags    DSK_WMH_MINHASH (0), or DSK_WMH_MINHASH_MANY: the float32 operation order of the
- *            reference's experimental minhash_many (:221-224; an all-zero row is None there, :241-245)
- *            | DSK_WMH_INPUT_LOG: d_v holds ln(weight) already (float32, NaN where the weight is zero) -- the host
+ *   d_out    [n, sample_size, 2] int64: (k, int(t_k)) per sample (:158); a non-finite t_k (a +inf weight, or a NaN
+ *            winner in MINHASH_MANY) is stored as INT64_MIN, numpy's float -> int64 cast on x86-64
+ *   d_status [n] int32: 0; 1 where the row has no candidate column: all zeros (reference: ValueError, :149-150), or
+ *            in minhash mode all zeros, negative or NaN (ValueError from np.nanargmin); 2 where t_k is not finite in
+ *            every sample (reference: OverflowError from int(t), :158)
+ *   flags    DSK_WMH_MINHASH (0): np.nanargmin, so negative and NaN weights are skipped like zeros;
+ *            or DSK_WMH_MINHASH_MANY: the float32 operation order of the reference's experimental minhash_many
+ *            (:221-224) and np.argmin over the non-zero columns, where the first negative or NaN weight wins (an
+ *            all-zero row is None there, :241-245)
+ *            | DSK_WMH_INPUT_LOG: d_v holds ln(weight) already (float32, -inf where the weight is zero) -- the host
  *            layer passes numpy's own float32 log (:152), which makes every step bit-identical to the reference;
- *            without it the kernel takes a correctly rounded log itself (<= 1 ulp from numpy's) */
+ *            without it the kernel takes log() in double rounded to float32 itself (the correctly rounded float32
+ *            log except within a few double ulps of a rounding midpoint; numpy's differs from it by up to 3 ulp) */
 #define DSK_WMH_MINHASH 0
 #define DSK_WMH_MINHASH_MANY 1
 #define DSK_WMH_INPUT_LOG 2

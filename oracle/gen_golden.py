@@ -2,7 +2,9 @@
 
 Run where an ekzhu/datasketch checkout exists (it imports the reference from it):
 
-    DATASKETCH_REF=<ekzhu/datasketch checkout> python oracle/gen_golden.py
+    DATASKETCH_REF=<ekzhu/datasketch checkout> python oracle/gen_golden.py [fixture ...]
+
+With fixture names (``wmh_special``, ``lsh``, ...) only those files are written.
 
 Every array written here is an output of the unmodified reference's public API
 (``MinHash``, ``LeanMinHash``, ``WeightedMinHashGenerator``, ``MinHashLSH``) on
@@ -193,6 +195,57 @@ def gen_wmh_many():
         d[f"{tag}_X"], d[f"{tag}_out"], d[f"{tag}_null"] = X, out, null
         d[f"{tag}_cfg"] = np.array([dim, ss, seed], dtype=np.int64)
     np.savez_compressed(os.path.join(OUT, "wmh_many.npz"), **d)
+
+
+WMH_SPECIAL_ROWS = [                               # dim 6: zero / -0.0 / negative / NaN / +-inf / subnormal / FLT_MAX
+    [1, 2, np.inf, 4, 0, 5],
+    [1, 2, -3, 4, 0, 5],
+    [1, 2, np.nan, 4, 0, 5],
+    [-1, -2, 0, 0, 0, 0],                          # all negative
+    [np.nan, np.nan, 0, 0, 0, np.nan],             # all NaN
+    [0, 0, 0, 0, 0, 0],                            # all zero
+    [-0.0, 1, 0, 2, -0.0, 3],
+    [1e-45, 1e-40, 1, 0, 3.4028235e38, 2],         # subnormals and FLT_MAX
+    [0, 0, 0, 0, 0, 1e-45],
+    [3.4028235e38, 0, 0, 0, 0, 0],
+    [-np.inf, 1, 2, 0, 3, 4],
+    [2, np.inf, 1, np.inf, 0, 3],                  # the first +inf wins
+    [1, np.nan, -1, 2, 0, np.inf],                 # NaN before a negative weight and +inf
+    [0, -5, 1, 1, np.inf, np.nan],
+    [1, 1, 1, 1, 1, 1],
+]
+
+
+def gen_wmh_special():
+    """WeightedMinHashGenerator.minhash (values, or the exception's type name) and minhash_many on rows holding zeros,
+    -0.0, negative, NaN, +-inf, subnormal and FLT_MAX weights, for two (sample_size, seed) choices."""
+    import warnings
+    d = {}
+    X = np.array(WMH_SPECIAL_ROWS, dtype=np.float32)
+    for dim, ss, seed, tag in [(6, 4, 1, "a"), (6, 16, 5, "b")]:
+        g = WeightedMinHashGenerator(dim, ss, seed)
+        out = np.zeros((len(X), ss, 2), dtype=np.int64)
+        err = []
+        for i, v in enumerate(X):
+            try:
+                with warnings.catch_warnings():
+                    warnings.simplefilter("ignore")
+                    out[i] = g.minhash(v).hashvalues
+                err.append("")
+            except Exception as e:  # noqa: BLE001  (the exception type is the expected value)
+                err.append(type(e).__name__)
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")
+            many = g.minhash_many(X)
+        many_out = np.zeros((len(X), ss, 2), dtype=np.int64)
+        for i, m in enumerate(many):
+            if m is not None:
+                many_out[i] = m.hashvalues
+        d[f"{tag}_cfg"] = np.array([dim, ss, seed], dtype=np.int64)
+        d[f"{tag}_out"], d[f"{tag}_err"] = out, np.array(err)
+        d[f"{tag}_many_out"], d[f"{tag}_many_null"] = many_out, np.array([m is None for m in many])
+    d["X"] = X
+    np.savez_compressed(os.path.join(OUT, "wmh_special.npz"), **d)
 
 
 def gen_ensemble():
@@ -441,17 +494,11 @@ def gen_storage_cassandra():
 
 if __name__ == "__main__":
     print("reference:", datasketch.__file__)
-    gen_minhash()
-    gen_lean()
-    gen_wmh()
-    gen_wmh_many()
-    gen_lsh()
-    gen_bbit()
-    gen_forest()
-    gen_ensemble()
-    gen_hashes()
-    gen_bloom()
-    gen_storage()
-    gen_storage_cassandra()
+    gens = {"minhash": gen_minhash, "lean": gen_lean, "wmh": gen_wmh, "wmh_many": gen_wmh_many,
+            "wmh_special": gen_wmh_special, "lsh": gen_lsh, "bbit": gen_bbit, "forest": gen_forest,
+            "ensemble": gen_ensemble, "hashes": gen_hashes, "bloom": gen_bloom, "storage": gen_storage,
+            "storage_cassandra": gen_storage_cassandra}
+    for name in sys.argv[1:] or gens:
+        gens[name]()
     for f in sorted(os.listdir(OUT)):
         print(f, os.path.getsize(os.path.join(OUT, f)))

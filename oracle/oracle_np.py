@@ -249,6 +249,55 @@ def wmh_minhash_many(X, rs: np.ndarray, ln_cs: np.ndarray, betas: np.ndarray) ->
     return ret
 
 
+INT64_MIN = np.iinfo(np.int64).min
+
+
+def wmh_from_log(vlog, rs: np.ndarray, ln_cs: np.ndarray, betas: np.ndarray, many: bool = False):
+    """([n, sample_size, 2] int64 of (k, t_k), [n] int32 status) for float32 logarithms ``vlog`` [n, dim]: the float32
+    step sequence of ``wmh_minhash`` (``many=False``) or ``wmh_minhash_many`` (``many=True``), vectorised over rows.
+
+    ``vlog`` is -inf where the weight is zero (``np.log(0)``); such columns are skipped in both modes.  A NaN log
+    (negative or NaN weight) is skipped by ``minhash``'s ``np.nanargmin`` and wins at its first occurrence in
+    ``minhash_many``'s ``np.argmin``.  A non-finite t_k is INT64_MIN (numpy's float -> int64 cast on x86-64).
+    status: 1 = no candidate column (the row is then all zeros), 2 = t_k not finite, else 0.
+    """
+    vlog = np.asarray(vlog, dtype=np.float32)
+    n, dim = vlog.shape
+    ss = rs.shape[0]
+    cand = vlog != -np.inf if many else ~(np.isnan(vlog) | (vlog == -np.inf))
+    out = np.zeros((n, ss, 2), dtype=np.int64)
+    nonfinite = np.zeros(n, dtype=bool)
+    rows = np.arange(n)
+    with np.errstate(invalid="ignore", over="ignore"):
+        for i in range(ss):
+            t = np.floor(vlog / rs[i] + betas[i])
+            if many:
+                ln_a = ln_cs[i] - (t - betas[i] + 1) * rs[i]
+            else:
+                ln_a = ln_cs[i] - (t - betas[i]) * rs[i] - rs[i]
+            k = np.argmin(np.where(cand, ln_a, np.float32(np.inf)), axis=1)   # NaN only where a NaN must win
+            tk = t[rows, k]
+            fin = np.isfinite(tk)
+            nonfinite |= ~fin
+            out[:, i, 0] = k
+            out[:, i, 1] = np.where(fin, np.where(fin, tk, 0).astype(np.int64), INT64_MIN)
+    empty = ~cand.any(axis=1)
+    out[empty] = 0
+    status = np.where(empty, 1, np.where(nonfinite, 2, 0)).astype(np.int32)
+    return out, status
+
+
+def wmh_terms64(vlog, r, ln_c, beta, many: bool = False):
+    """(floor argument, ln_a) in float64 from the same float32 parameters: ``vlog / r + beta`` and ``ln_a`` evaluated
+    without float32 rounding (arrays broadcast).  Used to show that a (k, t) difference between two float32
+    evaluations is a real near-tie: two ln_a a few float32 ulps apart, or a floor argument that close to an integer."""
+    vlog, r, ln_c, beta = (np.asarray(x, dtype=np.float64) for x in (vlog, r, ln_c, beta))
+    arg = vlog / r + beta
+    t = np.floor(arg)
+    ln_a = ln_c - (t - beta + 1) * r if many else ln_c - (t - beta) * r - r
+    return arg, ln_a
+
+
 def wmh_jaccard(hv1: np.ndarray, hv2: np.ndarray) -> float:
     """Fraction of samples with equal (k,t) rows (datasketch/weighted_minhash.py:55-60)."""
     inter = 0

@@ -520,6 +520,166 @@ def test_wmh_kernel_both_formulas(emu, golden, tag):
             assert not status.any() and np.array_equal(out, want)
 
 
+# ---- wmh_kernel edges: ties across the unroll quad / tile / remainder loop, ss > 128, floor edges, special weights ----
+WMH_MANY, WMH_INPUT_LOG = 1, 2
+
+
+def _np_log32(V):
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.log(np.asarray(V, dtype=np.float32))
+
+
+def _emu_wmh(lib, par, V, flags):
+    rs_, ln_cs, betas = (np.ascontiguousarray(x, dtype=np.float32) for x in par)
+    ss, dim = rs_.shape
+    V = np.ascontiguousarray(V, dtype=np.float32)
+    out = np.full((len(V), ss, 2), -7, dtype=np.int64)
+    status = np.full(len(V), -7, dtype=np.int32)
+    assert lib.emu_wmh(_ptr(rs_), _ptr(ln_cs), _ptr(betas), ss, dim, _ptr(V), ctypes.c_int64(len(V)), _ptr(out),
+                       _ptr(status), flags) == 0
+    return out, status
+
+
+def _wmh_oracle_for(V, par, flags):
+    """What the kernel must return for weights V under ``flags``: with DSK_WMH_INPUT_LOG the kernel gets numpy's log;
+    without it, the float64 log rounded to float32 (the device's log(); glibc's here)."""
+    V = np.asarray(V, dtype=np.float32)
+    if flags & WMH_INPUT_LOG:
+        vlog = _np_log32(V)
+    else:
+        with np.errstate(divide="ignore", invalid="ignore"):
+            vlog = np.log(V.astype(np.float64)).astype(np.float32)
+    return o.wmh_from_log(vlog, *par, many=bool(flags & WMH_MANY))
+
+
+def _wmh_feed(V, flags):
+    return _np_log32(V) if flags & WMH_INPUT_LOG else np.asarray(V, dtype=np.float32)
+
+
+WMH_TIE_PAIRS = [(0, 1), (3, 4), (255, 256), (260, 261)]   # one unroll quad, across quads, across the tile, remainder
+
+
+def _wmh_tie_case(dim=263, ss=130, seed=21):
+    """Parameters with column j a copy of column i for each tie pair, and rows in which every sample ties i with j."""
+    rs_, ln_cs, betas = (x.copy() for x in o.wmh_params(dim, ss, seed))
+    for i, j in WMH_TIE_PAIRS:
+        rs_[:, j], ln_cs[:, j], betas[:, j] = rs_[:, i], ln_cs[:, i], betas[:, i]
+    rng = np.random.RandomState(seed)
+    rows = []
+    for i, j in WMH_TIE_PAIRS:
+        v = np.zeros(dim, np.float32)
+        v[i] = v[j] = rng.uniform(0.5, 5)
+        rows.append(v)
+    v = rng.uniform(0.1, 2, dim).astype(np.float32)             # everything non-zero, the tied pairs heavy
+    for i, j in WMH_TIE_PAIRS:
+        v[i] = v[j] = 1e4
+    rows.append(v)
+    v = np.zeros(dim, np.float32)
+    v[dim - 1] = 3.0                                             # only the last column of the last tile
+    rows.append(v)
+    return (rs_, ln_cs, betas), np.stack(rows)
+
+
+@pytest.mark.parametrize("flags", [0, WMH_MANY, WMH_INPUT_LOG, WMH_MANY | WMH_INPUT_LOG])
+def test_wmh_kernel_ties_first_index(emu, flags):
+    """Equal ln_a at columns i < j (identical parameters and weight) gives k = i, inside one 4-dim unroll quad, across
+    quads, across the 256-dim tile and inside the remainder loop; a row whose only weight is the last column works.
+    ss = 130 also runs the second sample slice (blockIdx.y = 1)."""
+    par, V = _wmh_tie_case()
+    out, st = _emu_wmh(emu.lib, par, _wmh_feed(V, flags), flags)
+    want, wst = _wmh_oracle_for(V, par, flags)
+    assert np.array_equal(st, wst) and not st.any()
+    assert np.array_equal(out, want)
+    for row, (i, j) in enumerate(WMH_TIE_PAIRS):
+        assert (out[row, :, 0] == i).all(), (i, j)
+    heavy = out[len(WMH_TIE_PAIRS), :, 0]
+    assert not np.isin(heavy, [j for _, j in WMH_TIE_PAIRS]).any()
+    assert np.isin(heavy, [i for i, _ in WMH_TIE_PAIRS]).mean() > 0.5
+    assert (out[-1, :, 0] == V.shape[1] - 1).all()
+
+
+@pytest.mark.parametrize("dim,ss", [(1, 1), (3, 129), (5, 33), (257, 200), (259, 31)])
+def test_wmh_kernel_shapes_exact(emu, dim, ss):
+    """Remainder-loop dims (dim % 4 != 0), the tile edge and sample counts past one 128-thread slice, in both modes and
+    with both log sources, equal to the oracle exactly."""
+    rng = np.random.RandomState(dim * 1000 + ss)
+    V = (rng.lognormal(0, 2, (9, dim)) * (rng.rand(9, dim) < 0.7)).astype(np.float32)
+    V[:, dim - 1] += 0.5                                         # no empty row
+    par = o.wmh_params(dim, ss, 3)
+    for flags in (0, WMH_MANY, WMH_INPUT_LOG, WMH_MANY | WMH_INPUT_LOG):
+        out, st = _emu_wmh(emu.lib, par, _wmh_feed(V, flags), flags)
+        want, wst = _wmh_oracle_for(V, par, flags)
+        assert np.array_equal(st, wst) and np.array_equal(out, want), flags
+
+
+def test_wmh_kernel_grid_stride_over_groups(emu):
+    """More vector groups than the launch's CTAs (the emulation's sm_count = 2 caps the grid at 16 groups of 8), so
+    the CTAs loop over groups: every row, the last partial group included, equals the oracle."""
+    n, dim, ss = 16 * 8 * 2 + 3, 5, 3
+    rng = np.random.RandomState(5)
+    V = rng.uniform(0, 4, (n, dim)).astype(np.float32)
+    V[V < 1] = 0
+    V[::17] = 0                                                  # empty rows -> status 1
+    par = o.wmh_params(dim, ss, 8)
+    for flags in (WMH_INPUT_LOG, WMH_MANY | WMH_INPUT_LOG):
+        out, st = _emu_wmh(emu.lib, par, _wmh_feed(V, flags), flags)
+        want, wst = _wmh_oracle_for(V, par, flags)
+        assert (wst == 1).sum() >= 16 and np.array_equal(st, wst) and np.array_equal(out, want)
+
+
+def _wmh_floor_case(ss=4):
+    """Exactly representable r and beta, and logarithms that make vlog / r + beta an exact integer, or one float32 ulp of
+    vlog either side of it."""
+    rvals = np.array([0.5, 0.75, 1.25, 2.0, 0.375, 3.0], np.float32)
+    bvals = np.array([0.25, 0.5, 0.125, 0.75, 0.0, 0.875], np.float32)
+    dim = len(rvals)
+    rs_ = np.tile(rvals, (ss, 1))
+    betas = np.tile(bvals, (ss, 1))
+    ln_cs = o.wmh_params(dim, ss, 4)[1].copy()
+    rows = []
+    for m in (-3, 0, 1, 4, 17):
+        exact = ((np.float32(m) - bvals) * rvals).astype(np.float32)   # dyadic: no rounding
+        assert np.array_equal(exact / rvals + bvals, np.full(dim, m, np.float32))
+        rows += [exact, np.nextafter(exact, np.float32(np.inf)), np.nextafter(exact, np.float32(-np.inf))]
+    return (rs_, ln_cs, betas), np.stack(rows).astype(np.float32)
+
+
+@pytest.mark.parametrize("many", [0, WMH_MANY])
+def test_wmh_kernel_floor_edges(emu, many):
+    par, vlog = _wmh_floor_case()
+    out, st = _emu_wmh(emu.lib, par, vlog, many | WMH_INPUT_LOG)
+    want, wst = o.wmh_from_log(vlog, *par, many=bool(many))
+    assert np.array_equal(st, wst) and not st.any() and np.array_equal(out, want)
+    t_exact = want[0::3, :, 1]
+    assert (want[2::3, :, 1] != t_exact).any()                  # one ulp below the integer drops t by one somewhere
+
+
+@pytest.mark.parametrize("tag", ["a", "b"])
+@pytest.mark.parametrize("flags", [0, WMH_MANY, WMH_INPUT_LOG, WMH_MANY | WMH_INPUT_LOG])
+def test_wmh_kernel_special_weights(emu, golden, tag, flags):
+    """Zeros, -0.0, negative, NaN, +-inf, subnormal and FLT_MAX weights against the reference's own results: minhash
+    skips negative / NaN weights (status 1 where nothing is left: ValueError) and reports a +inf winner as status 2
+    (OverflowError); minhash_many lets the first negative / NaN weight win and stores a non-finite t as INT64_MIN."""
+    g = golden("wmh_special")
+    X = g["X"]
+    dim, ss, seed = (int(x) for x in g[f"{tag}_cfg"])
+    par = o.wmh_params(dim, ss, seed)
+    out, st = _emu_wmh(emu.lib, par, _wmh_feed(X, flags), flags)
+    want, wst = _wmh_oracle_for(X, par, flags)
+    assert np.array_equal(st, wst) and np.array_equal(out, want)
+    if flags & WMH_MANY:
+        null = g[f"{tag}_many_null"]
+        assert np.array_equal(st == 1, null)
+        if flags & WMH_INPUT_LOG:
+            assert np.array_equal(out, g[f"{tag}_many_out"])
+    else:
+        err = g[f"{tag}_err"]
+        assert np.array_equal(st == 1, err == "ValueError") and np.array_equal(st == 2, err == "OverflowError")
+        assert (out[st == 2][:, :, 1] == np.iinfo(np.int64).min).all()
+        if flags & WMH_INPUT_LOG:
+            assert np.array_equal(out[err == ""], g[f"{tag}_out"][err == ""])
+
+
 # ---- randomised differential run ---------------------------------------------------------------------------------------
 def _fuzz_signature_kernel(run, seed, iterations):
     """Random num_perm / document shapes / token kinds / modes / init forms / unit and grid sizes;

@@ -177,6 +177,72 @@ def test_wmh_minhash_many(golden):
         o.wmh_minhash_many(np.ones((2, 3)), *o.wmh_params(5, 4, 1))
 
 
+def _np_log32(V):
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.log(np.asarray(V, dtype=np.float32))
+
+
+def test_wmh_from_log(golden):
+    """The vectorised float32 step sequence equals the per-vector restatements and the reference's own outputs,
+    including the special-weight rows (zeros, -0.0, negative, NaN, +-inf, subnormals, FLT_MAX) of wmh_special."""
+    g = golden("wmh")
+    for tag in ("small", "tiny", "c4"):
+        dim, ss, seed = (int(x) for x in g[f"{tag}_cfg"])
+        out, st = o.wmh_from_log(_np_log32(g[f"{tag}_v"]), *o.wmh_params(dim, ss, seed))
+        assert not st.any() and np.array_equal(out, g[f"{tag}_out"])
+    g = golden("wmh_many")
+    for tag in ("small", "tiny", "mid"):
+        dim, ss, seed = (int(x) for x in g[f"{tag}_cfg"])
+        out, st = o.wmh_from_log(_np_log32(g[f"{tag}_X"]), *o.wmh_params(dim, ss, seed), many=True)
+        null = g[f"{tag}_null"]
+        assert np.array_equal(st == 1, null) and not (st == 2).any()
+        assert np.array_equal(out[~null], g[f"{tag}_out"][~null]) and not out[null].any()
+    rs = np.random.RandomState(3)
+    V = (rs.lognormal(0, 3, (40, 259)) * (rs.rand(40, 259) < 0.6)).astype(np.float32)
+    V[:, 7] = 1.0
+    par = o.wmh_params(259, 37, 9)
+    out, st = o.wmh_from_log(_np_log32(V), *par)
+    assert not st.any() and np.array_equal(out, np.stack([o.wmh_minhash(v, *par) for v in V]))
+    out, st = o.wmh_from_log(_np_log32(V), *par, many=True)
+    assert not st.any() and np.array_equal(out, np.stack(o.wmh_minhash_many(V, *par)))
+    g = golden("wmh_special")
+    X = g["X"]
+    for tag in ("a", "b"):
+        dim, ss, seed = (int(x) for x in g[f"{tag}_cfg"])
+        par = o.wmh_params(dim, ss, seed)
+        out, st = o.wmh_from_log(_np_log32(X), *par)
+        err = g[f"{tag}_err"]
+        assert np.array_equal(st == 1, err == "ValueError") and np.array_equal(st == 2, err == "OverflowError")
+        ok = err == ""
+        assert ok.sum() >= 5 and np.array_equal(out[ok], g[f"{tag}_out"][ok])
+        out, st = o.wmh_from_log(_np_log32(X), *par, many=True)
+        null = g[f"{tag}_many_null"]
+        assert np.array_equal(st == 1, null) and (st == 2).sum() >= 5
+        assert np.array_equal(out, g[f"{tag}_many_out"])
+        with np.errstate(invalid="ignore"):
+            per_row = o.wmh_minhash_many(X, *par)
+        assert [m is None for m in per_row] == null.tolist()
+        assert all(np.array_equal(m, out[i]) for i, m in enumerate(per_row) if m is not None)
+
+
+def test_wmh_terms64():
+    """The float64 evaluation agrees with the float32 one to a few float32 ulps, and exactly on exact inputs."""
+    rs, ln_cs, betas = o.wmh_params(50, 8, 2)
+    vlog = _np_log32(np.random.RandomState(0).uniform(0.1, 10, 50))
+    for many in (False, True):
+        arg, ln_a = o.wmh_terms64(vlog, rs, ln_cs, betas, many)
+        arg32 = vlog / rs + betas
+        t = np.floor(arg32)
+        ln_a32 = ln_cs - (t - betas + 1) * rs if many else ln_cs - (t - betas) * rs - rs
+        same_t = np.floor(arg) == t
+        scale_arg = np.abs(vlog / rs) + betas                     # float32 rounding is relative to the operands
+        scale_ln_a = np.abs(ln_cs) + np.abs(t - betas + 1) * rs + rs
+        assert same_t.mean() > 0.99 and np.all(np.abs(arg - arg32) <= 2 * np.spacing(scale_arg))
+        assert np.all((np.abs(ln_a - ln_a32) <= 4 * np.spacing(scale_ln_a))[same_t])
+    arg, ln_a = o.wmh_terms64(np.float32(3.0), np.float32(2.0), np.float32(0.5), np.float32(0.25))
+    assert arg == 1.75 and ln_a == 0.5 - (1.0 - 0.25) * 2.0 - 2.0
+
+
 def test_token_hashes(golden):
     """xxh32 restatement vs the values the `xxhash` package produced; MurmurHash3 x86_32 vs published vectors
     (SMHasher / mmh3 documentation); the product's single-token host functions agree with both."""

@@ -47,7 +47,8 @@ def test_wmh_matches_reference_fixture(dsk, golden, tag):
     got = gen.minhash_batch(V)
     assert got.dtype == np.int64 and got.shape == want.shape
     n_diff = int((got != want).any(axis=2).sum())
-    # exact on the fixtures (the only non-IEEE step is log, <= 1 ulp); any difference must be a near-tie
+    # the fixtures were made on another host, whose numpy float32 log may round differently: any difference must be a
+    # near-tie
     for u in range(len(V)):
         if (got[u] != want[u]).any():
             assert _explain_mismatch(V[u], rs, ln_cs, betas, got[u], want[u]) == []
