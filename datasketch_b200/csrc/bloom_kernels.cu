@@ -24,27 +24,35 @@ __device__ __forceinline__ uint64_t bloom_mix(uint64_t h) {
     return h;
 }
 
-// warp <-> document: the row is read once with coalesced loads into shared memory, then lane j sums band j.
+// warp <-> document: the b*r values the bands use are read once with coalesced loads into the warp's slice of shared
+// memory (STAGED), then lane j sums band j.  A row too long for shared memory is summed straight from global memory.
 // x < 2^32 * r, so the uint64 sum cannot wrap for r <= 2^32 and `% p` is the conditional fold below.
-template <int MODE>   // 0 = write the keys, 1 = insert into the tables, 2 = query the tables
+template <int MODE, bool STAGED>   // MODE 0 = write the keys, 1 = insert into the tables, 2 = query the tables
 __global__ void __launch_bounds__(256) bloom_bands_kernel(const uint32_t *__restrict__ sig, int64_t n, int k, int b, int r,
                                                           uint64_t *__restrict__ keys, uint32_t *__restrict__ bits,
                                                           uint64_t words_per_table, uint64_t n_bits, int n_hashes,
                                                           uint8_t *__restrict__ hit) {
     DSK_DYNAMIC_SMEM_T(uint32_t, s_row, 16);
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    uint32_t *row = s_row + (size_t)w * k;
     const int br = b * r;
+    uint32_t *row = s_row + (size_t)w * br;
     for (int64_t i = (int64_t)blockIdx.x * nw + w; i < n; i += (int64_t)gridDim.x * nw) {
         const uint32_t *g = sig + i * k;
-        __syncwarp();
-        for (int c = lane; c < br; c += 32) row[c] = __ldg(g + c);
-        __syncwarp();
+        if (STAGED) {
+            __syncwarp();
+            for (int c = lane; c < br; c += 32) row[c] = __ldg(g + c);
+            __syncwarp();
+        }
         bool any = false;
         for (int j = lane; j < b; j += 32) {
-            const uint32_t *v = row + j * r;
             uint64_t x = 0;
-            for (int q = 0; q < r; ++q) x += v[q];
+            if (STAGED) {
+                const uint32_t *v = row + j * r;
+                for (int q = 0; q < r; ++q) x += v[q];
+            } else {
+                const uint32_t *v = g + (int64_t)j * r;
+                for (int q = 0; q < r; ++q) x += __ldg(v + q);
+            }
             x = mod_p61(x);
             if (MODE == 0) {
                 keys[i * b + j] = x;
@@ -84,29 +92,40 @@ __global__ void __launch_bounds__(256) band_sums_kernel(const uint32_t *__restri
     }
 }
 
+template <int MODE>
+static cudaError_t launch_bloom_mode(int warps, size_t smem, const uint32_t *sig, int64_t n, int k, int b, int r,
+                                     uint64_t *keys, uint32_t *bits, uint64_t words_per_table, uint64_t n_bits,
+                                     int n_hashes, uint8_t *hit, int grid, cudaStream_t s) {
+    if (smem == 0) {
+        DSK_LAUNCH((bloom_bands_kernel<MODE, false>), grid, warps * 32, 0, s, sig, n, k, b, r, keys, bits, words_per_table, n_bits, n_hashes, hit);
+        return cudaGetLastError();
+    }
+    const cudaError_t e = cudaFuncSetAttribute(bloom_bands_kernel<MODE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    DSK_LAUNCH((bloom_bands_kernel<MODE, true>), grid, warps * 32, smem, s, sig, n, k, b, r, keys, bits, words_per_table, n_bits, n_hashes, hit);
+    return cudaGetLastError();
+}
+
+// Each warp stages the b*r values it sums (not the whole num_perm-long row): 8 warps per CTA while their slices fit in
+// 96 KB, fewer for longer rows.  A row longer than 96 KB (b*r > 24576) is read from global memory instead, as
+// band_sums_kernel does, so any b*r <= num_perm launches.
 static cudaError_t launch_bloom_bands(int mode, const uint32_t *sig, int64_t n, int k, int b, int r, uint64_t *keys,
                                       uint32_t *bits, uint64_t words_per_table, uint64_t n_bits, int n_hashes,
                                       uint8_t *hit, int sm_count, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
+    constexpr size_t kStageBytes = 96 * 1024;
+    const size_t row_bytes = (size_t)b * r * 4;
     int warps = 8;
-    while (warps > 1 && (size_t)warps * k * 4 > 96 * 1024) warps >>= 1;
-    const size_t smem = (size_t)warps * k * 4;
-    const int grid = (int)std::min<int64_t>((n + warps - 1) / warps, (int64_t)sm_count * 8);
-    cudaError_t e = cudaSuccess;
-    if (mode == 0) {
-        e = cudaFuncSetAttribute(bloom_bands_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        DSK_LAUNCH((bloom_bands_kernel<0>), grid, warps * 32, smem, s, sig, n, k, b, r, keys, bits, words_per_table, n_bits, n_hashes, hit);
-    } else if (mode == 1) {
-        e = cudaFuncSetAttribute(bloom_bands_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        DSK_LAUNCH((bloom_bands_kernel<1>), grid, warps * 32, smem, s, sig, n, k, b, r, keys, bits, words_per_table, n_bits, n_hashes, hit);
-    } else {
-        e = cudaFuncSetAttribute(bloom_bands_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        DSK_LAUNCH((bloom_bands_kernel<2>), grid, warps * 32, smem, s, sig, n, k, b, r, keys, bits, words_per_table, n_bits, n_hashes, hit);
+    while (warps > 1 && warps * row_bytes > kStageBytes) warps >>= 1;
+    size_t smem = warps * row_bytes;
+    if (smem > kStageBytes) {
+        warps = 8;
+        smem = 0;
     }
-    return cudaGetLastError();
+    const int grid = (int)std::min<int64_t>((n + warps - 1) / warps, (int64_t)sm_count * 8);
+    if (mode == 0) return launch_bloom_mode<0>(warps, smem, sig, n, k, b, r, keys, bits, words_per_table, n_bits, n_hashes, hit, grid, s);
+    if (mode == 1) return launch_bloom_mode<1>(warps, smem, sig, n, k, b, r, keys, bits, words_per_table, n_bits, n_hashes, hit, grid, s);
+    return launch_bloom_mode<2>(warps, smem, sig, n, k, b, r, keys, bits, words_per_table, n_bits, n_hashes, hit, grid, s);
 }
 
 cudaError_t launch_band_sums(const uint32_t *sig, int64_t n, int k, int b, int r, uint64_t *keys, int sm_count, cudaStream_t s) {

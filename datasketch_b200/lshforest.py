@@ -171,6 +171,8 @@ class GpuLSHForest:
             sig = torch.from_numpy(_signature_matrix(sig).view(np.int32)).cuda(self.device)
         if sig.dim() != 2 or sig.shape[1] < self.k * self.l or sig.shape[1] != self.h:
             raise ValueError("The num_perm of MinHash out of range")
+        if sig.element_size() != 4:
+            raise TypeError("GpuLSHForest takes the 32-bit signature matrix")
         self._blocks.append(sig.contiguous())
         if keys is not None:
             self.keys.extend(keys)
@@ -215,6 +217,8 @@ class GpuLSHForest:
             sig = torch.from_numpy(_signature_matrix(sig).view(np.int32)).cuda(self.device)
         if sig.dim() != 2 or sig.shape[1] != self.h:
             raise ValueError("The num_perm of MinHash out of range")
+        if sig.element_size() != 4:
+            raise TypeError("GpuLSHForest takes the 32-bit signature matrix")
         sig = sig.contiguous()
         nq, n = sig.shape[0], self._sig.shape[0]
         out = torch.empty((nq, k), dtype=torch.int32, device=sig.device)
