@@ -1398,6 +1398,103 @@ int dsk_lsh_ensemble_query_fill(const dsk_lsh_ensemble *e, const uint32_t *d_qsi
     return DSK_OK;
 }
 
+// ---- MinHashLSHEnsemble's size partitioner -------------------------------------------------------------------------------
+// acc += a * b rounded up to 256 bytes; false if it does not fit in size_t
+static bool ws_add(size_t &acc, uint64_t a, uint64_t b) {
+    if (a != 0 && b > (SIZE_MAX - 512) / a) return false;
+    const size_t part = (size_t)((a * b + 255) / 256 * 256);
+    if (acc > SIZE_MAX - part) return false;
+    acc += part;
+    return true;
+}
+
+// workspace layout: sizes, counts [n] int64; the terms rows of the cost launch (large n); for 2 <= num_part < n the triangle
+// [n(n+1)/2], the tables [num_part - 1][n] (doubles) and the upper indices [num_part] int64
+static size_t partition_ws(int64_t n, int num_part, size_t *off_terms, size_t *off_cost, size_t *off_tab, size_t *off_upper) {
+    size_t acc = 0;
+    bool ok = ws_add(acc, (uint64_t)n, 16);
+    if (off_terms) *off_terms = acc;
+    ok = ok && ws_add(acc, (uint64_t)partition_term_rows(n), (uint64_t)n * 8);
+    if (num_part >= 2 && num_part < n) {
+        if (off_cost) *off_cost = acc;
+        ok = ok && (uint64_t)n < (1ull << 32) && ws_add(acc, (uint64_t)n * (uint64_t)(n + 1) / 2, 8);
+        if (off_tab) *off_tab = acc;
+        ok = ok && ws_add(acc, (uint64_t)(num_part - 1) * 8, (uint64_t)n);
+        if (off_upper) *off_upper = acc;
+        ok = ok && ws_add(acc, (uint64_t)num_part, 8);
+    }
+    return ok ? acc : SIZE_MAX;
+}
+
+size_t dsk_ensemble_partition_workspace_size(int64_t n_sizes, int num_part) {
+    if (n_sizes < 1 || num_part < 1) return 0;
+    return partition_ws(n_sizes, num_part, nullptr, nullptr, nullptr, nullptr);
+}
+
+int dsk_ensemble_partition(const int64_t *h_sizes, const int64_t *h_counts, int64_t n_sizes, int num_part, void *d_workspace,
+                           size_t workspace_bytes, int device, int64_t *h_upper_idx, double *d_cost, void *stream) {
+    const char *who = "dsk_ensemble_partition";
+    if (n_sizes < 1 || num_part < 1) {
+        set_error("%s: need n_sizes >= 1 and num_part >= 1 (got %lld and %d)", who, (long long)n_sizes, num_part);
+        return DSK_ERR_INVALID;
+    }
+    if (!h_sizes || !h_counts || !h_upper_idx) {
+        set_error("%s: null buffer", who);
+        return DSK_ERR_INVALID;
+    }
+    const int64_t kMax = (int64_t)1 << 62;
+    for (int64_t i = 0; i < n_sizes; ++i) {
+        if (h_sizes[i] <= 0 || h_sizes[i] >= kMax || (i > 0 && h_sizes[i] <= h_sizes[i - 1])) {
+            set_error("%s: sizes must be strictly ascending, each in [1, 2^62) (sizes[%lld] = %lld)", who, (long long)i,
+                      (long long)h_sizes[i]);
+            return DSK_ERR_INVALID;
+        }
+        if (h_counts[i] <= 0 || h_counts[i] >= kMax) {
+            set_error("%s: counts must be in [1, 2^62) (counts[%lld] = %lld)", who, (long long)i, (long long)h_counts[i]);
+            return DSK_ERR_INVALID;
+        }
+    }
+    const bool trivial = num_part < 2 || num_part >= n_sizes;
+    if (trivial) {   // one partition, or one per size: no table (the triangle only if asked for)
+        if (num_part < 2) h_upper_idx[0] = n_sizes - 1;
+        else for (int64_t i = 0; i < n_sizes; ++i) h_upper_idx[i] = i;
+        if (!d_cost) return DSK_OK;
+    }
+    size_t off_terms = 0, off_cost = 0, off_tab = 0, off_upper = 0;
+    const size_t need = partition_ws(n_sizes, num_part, &off_terms, &off_cost, &off_tab, &off_upper);
+    if (need == SIZE_MAX) {
+        set_error("%s: the workspace for n_sizes = %lld and num_part = %d does not fit in size_t", who, (long long)n_sizes,
+                  num_part);
+        return DSK_ERR_INVALID;
+    }
+    if (!d_workspace || workspace_bytes < need || ((uintptr_t)d_workspace & 15u) != 0) {
+        set_error("%s: the workspace must be 16-byte aligned and hold %zu bytes (got %zu at %p)", who, need, workspace_bytes,
+                  d_workspace);
+        return DSK_ERR_INVALID;
+    }
+    if (d_cost && ((uintptr_t)d_cost & 7u) != 0) {
+        set_error("%s: d_cost must be 8-byte aligned", who);
+        return DSK_ERR_INVALID;
+    }
+    DevInfo *dev;
+    int rc = get_dev(device, &dev);
+    if (rc) return rc;
+    DevGuard guard(device);
+    const cudaStream_t s = (cudaStream_t)stream;
+    unsigned char *ws = static_cast<unsigned char *>(d_workspace);
+    int64_t *sizes = reinterpret_cast<int64_t *>(ws), *counts = sizes + n_sizes;
+    double *g_terms = partition_term_rows(n_sizes) ? reinterpret_cast<double *>(ws + off_terms) : nullptr;
+    double *cost = d_cost ? d_cost : reinterpret_cast<double *>(ws + off_cost);
+    double *tab = trivial ? nullptr : reinterpret_cast<double *>(ws + off_tab);
+    int64_t *upper = reinterpret_cast<int64_t *>(ws + off_upper);
+    DSK_CUDA(cudaMemcpyAsync(sizes, h_sizes, (size_t)n_sizes * 8, cudaMemcpyHostToDevice, s));
+    DSK_CUDA(cudaMemcpyAsync(counts, h_counts, (size_t)n_sizes * 8, cudaMemcpyHostToDevice, s));
+    DSK_CUDA(ensemble_partition(sizes, counts, n_sizes, num_part, cost, tab, g_terms, upper, dev->sm_count, s));
+    if (!trivial) DSK_CUDA(cudaMemcpyAsync(h_upper_idx, upper, (size_t)num_part * 8, cudaMemcpyDeviceToHost, s));
+    DSK_CUDA(cudaStreamSynchronize(s));
+    return DSK_OK;
+}
+
 int dsk_jaccard_pairs(const uint32_t *d_sig, int64_t n_rows, int num_perm, const int64_t *d_i, const int64_t *d_j,
                       int64_t m, int32_t *d_count, void *stream) {
     if (n_rows < 0 || num_perm <= 0 || m < 0 || (m > 0 && (!d_sig || !d_i || !d_j || !d_count))) {

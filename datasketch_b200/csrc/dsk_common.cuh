@@ -18,6 +18,13 @@
 #define DSK_LAUNCH(kernel, grid, block, smem, stream, ...) ::emu_launch(kernel, grid, block, smem, __VA_ARGS__)
 #define DSK_DYNAMIC_SMEM(name) unsigned char *name = ::emu_dynamic_smem()
 #define DSK_DYNAMIC_SMEM_T(type, name, align) type *name = reinterpret_cast<type *>(::emu_dynamic_smem())
+// float64 operations rounded one by one, as the size partitioner uses them (the emulation is built with -ffp-contract=off;
+// x86-64 SSE2 arithmetic is IEEE binary64 with round to nearest even, and so is the int64 -> double conversion)
+static inline double __dadd_rn(double a, double b) { return a + b; }
+static inline double __dsub_rn(double a, double b) { return a - b; }
+static inline double __dmul_rn(double a, double b) { return a * b; }
+static inline double __ddiv_rn(double a, double b) { return a / b; }
+static inline double __ll2double_rn(long long v) { return (double)v; }
 #else
 #define DSK_LAUNCH(kernel, grid, block, smem, stream, ...) kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
 #define DSK_DYNAMIC_SMEM(name) extern __shared__ __align__(128) unsigned char name[]
@@ -181,6 +188,13 @@ cudaError_t ensemble_index(const EnsembleDev &en, const uint32_t *rows, const in
                            cudaStream_t s);
 cudaError_t ensemble_query(const EnsembleDev &en, const uint32_t *qsig, int64_t nq, const int32_t *sel, int64_t *counts,
                            const int64_t *ptr, int32_t *idx, int32_t *eq, int sm_count, cudaStream_t s);
+// the size partitioner over n distinct sizes (device copies of sizes / counts): the cost triangle, and with tab != nullptr
+// (2 <= num_part < n; num_part - 1 rows of n doubles) the dynamic programme and the upper index of each partition into
+// upper[num_part].  g_terms: partition_term_rows(n) rows of n doubles (none while a column's terms fit shared memory).
+bool partition_terms_in_smem(int64_t n);
+int64_t partition_term_rows(int64_t n);
+cudaError_t ensemble_partition(const int64_t *sizes, const int64_t *counts, int64_t n, int num_part, double *cost, double *tab,
+                               double *g_terms, int64_t *upper, int sm_count, cudaStream_t s);
 
 cudaError_t launch_jaccard_pairs(const uint32_t *sig, int64_t n_rows, int k, const int64_t *ia, const int64_t *ib,
                                  int64_t m, int32_t *out, int sm_count, cudaStream_t s);

@@ -1330,3 +1330,195 @@ cudaError_t ensemble_query(const EnsembleDev &en, const uint32_t *qsig, int64_t 
 }
 
 }  // namespace dsk
+
+// ---- MinHashLSHEnsemble's size partitioner (lshensemble.py:81-120 = lshensemble_partition.py:54-196) ----------------------
+// Over the D distinct set sizes (ascending) with their counts: cost[l, u] = sum over i in [l, u] of
+// (sizes[u] - sizes[i]) / sizes[u] * counts[i], as numpy evaluates it (each operation rounded on its own, the sum numpy's
+// float64 pairwise sum), stored as a column-major upper triangle (entry (l, u) at u(u+1)/2 + l); then the reference's dynamic
+// programme over p = 2 .. num_part-1 intervals and its back-tracking, every argmin taking the first index among equal values.
+// The triangle is D^3/6 additions and D^2/2 divisions; the programme and the back-tracking read it num_part times.
+namespace dsk {
+
+// numpy's pairwise_sum of a[0..n) for n <= 128 (a leaf): below 8 elements a sequential sum from 0.0; else eight accumulators
+// seeded with a[0..8) and stepping by 8, combined ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), then the n mod 8 tail in order
+__device__ __forceinline__ double np_leaf_sum(const double *a, int n) {
+    if (n < 8) {
+        double res = 0.0;
+        for (int i = 0; i < n; ++i) res = __dadd_rn(res, a[i]);
+        return res;
+    }
+    double r0 = a[0], r1 = a[1], r2 = a[2], r3 = a[3], r4 = a[4], r5 = a[5], r6 = a[6], r7 = a[7];
+    const int m = n - n % 8;
+    for (int i = 8; i < m; i += 8) {
+        r0 = __dadd_rn(r0, a[i]);
+        r1 = __dadd_rn(r1, a[i + 1]);
+        r2 = __dadd_rn(r2, a[i + 2]);
+        r3 = __dadd_rn(r3, a[i + 3]);
+        r4 = __dadd_rn(r4, a[i + 4]);
+        r5 = __dadd_rn(r5, a[i + 5]);
+        r6 = __dadd_rn(r6, a[i + 6]);
+        r7 = __dadd_rn(r7, a[i + 7]);
+    }
+    double res = __dadd_rn(__dadd_rn(__dadd_rn(r0, r1), __dadd_rn(r2, r3)), __dadd_rn(__dadd_rn(r4, r5), __dadd_rn(r6, r7)));
+    for (int i = m; i < n; ++i) res = __dadd_rn(res, a[i]);
+    return res;
+}
+
+// numpy's pairwise_sum of a[0..n): above 128 elements, the sum of the first n2 = n/2 - (n/2) % 8 plus the sum of the rest.
+// The recursion runs on an explicit stack, left half first, so the leaves are met in ascending order: pos is where the next
+// one starts, rest[d] the length of level d's right half while its left half is summed (-1 once it is summed into left[d]).
+constexpr int kPairwiseDepth = 48;   // each level at least halves n - 8: enough for any n < 2^48
+__device__ __forceinline__ double np_pairwise_sum(const double *a, int64_t n) {
+    int64_t rest[kPairwiseDepth];
+    double left[kPairwiseDepth];
+    int depth = 0;
+    int64_t pos = 0;
+    while (true) {
+        while (n > 128) {
+            int64_t n2 = n / 2;
+            n2 -= n2 % 8;
+            rest[depth++] = n - n2;
+            n = n2;
+        }
+        double v = np_leaf_sum(a + pos, (int)n);
+        pos += n;
+        while (depth > 0 && rest[depth - 1] < 0) v = __dadd_rn(left[--depth], v);
+        if (depth == 0) return v;
+        left[depth - 1] = v;
+        n = rest[depth - 1];
+        rest[depth - 1] = -1;
+    }
+}
+
+constexpr int kPartitionCostThreads = 512;
+constexpr int64_t kPartitionSmemTerms = 28 * 1024;    // a column's terms fit the shared memory of one CTA up to D = 28672
+constexpr int64_t kPartitionTermRows = 512;           // beyond that: CTAs of the cost launch, one global row of D terms each
+
+// CTA <-> column u (largest first, grid-stride): the u + 1 terms of the column, term i = (sizes[u] - sizes[i]) / sizes[u] *
+// counts[i] (every operation rounded on its own: no contraction into an FMA, no reciprocal), into shared memory (or the CTA's
+// row of g_terms), then thread <-> entry l: cost[l, u] = the pairwise sum of terms l..u.  row0[u] = cost[0, u] (if not null).
+template <bool SMEM_TERMS>
+__global__ void __launch_bounds__(kPartitionCostThreads) partition_cost_kernel(const int64_t *__restrict__ sizes,
+                                                                               const int64_t *__restrict__ counts, int64_t n,
+                                                                               double *__restrict__ cost,
+                                                                               double *__restrict__ row0, double *g_terms) {
+    DSK_DYNAMIC_SMEM_T(double, s_terms, 16);
+    double *t = SMEM_TERMS ? s_terms : g_terms + (int64_t)blockIdx.x * n;
+    for (int64_t u = n - 1 - blockIdx.x; u >= 0; u -= gridDim.x) {
+        const double top = __ll2double_rn(sizes[u]);
+        __syncthreads();   // the previous column's sums are done with t
+        for (int64_t i = threadIdx.x; i <= u; i += blockDim.x)
+            t[i] = __dmul_rn(__ddiv_rn(__dsub_rn(top, __ll2double_rn(sizes[i])), top), __ll2double_rn(counts[i]));
+        __syncthreads();
+        double *col = cost + u * (u + 1) / 2;
+        for (int64_t l = threadIdx.x; l <= u; l += blockDim.x) {
+            const double v = np_pairwise_sum(t + l, u - l + 1);
+            col[l] = v;
+            if (l == 0 && row0) row0[u] = v;
+        }
+    }
+}
+
+// warp <-> u in [p-1, n): tab[u] = min over u1 in [p-2, u-1] of prev[u1] + cost[u1 + 1, u] (column u is contiguous).  Entries
+// u < p-1 are not written (the caller zeroes them, as the reference's zero-initialised matrix).
+__global__ void __launch_bounds__(256) partition_dp_kernel(const double *__restrict__ cost, const double *__restrict__ prev,
+                                                           double *__restrict__ tab, int p, int64_t n) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    for (int64_t u = n - 1 - ((int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)); u >= p - 1; u -= warps) {
+        const double *col = cost + u * (u + 1) / 2 + 1;   // col[u1] = cost[u1 + 1, u]
+        double best = (double)INFINITY;
+        for (int64_t u1 = p - 2 + lane; u1 < u; u1 += 32) {
+            const double v = __dadd_rn(prev[u1], col[u1]);
+            best = v < best ? v : best;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const double w = __shfl_xor_sync(0xFFFFFFFFu, best, o);
+            best = w < best ? w : best;
+        }
+        if (lane == 0) tab[u] = best;
+    }
+}
+
+// (v, i) pairs: the smaller value, the smaller index among equal values
+__device__ __forceinline__ void argmin_first(double &v, int64_t &i, double w, int64_t j) {
+    if (w < v || (w == v && j < i)) { v = w; i = j; }
+}
+
+// one CTA: the reference's back-tracking.  u = n-1; for p = num_part .. 2: u1 = the first argmin over [p-2, u-1] of
+// prev[u1] + cost[u1 + 1, u], the upper index of partition p-2, then u = u1.  prev is the (p-1)-interval table for the
+// first step and, as in the reference (lshensemble_partition.py:158-166), the p-interval table after it, where the
+// recurrence used p-1; its entries below p-1 are the zeros.  tab row q (q = 1 .. num_part-1) is the q-interval table at
+// tab + (q-1) * n, row 1 = cost[0, .].
+__global__ void __launch_bounds__(256) partition_backtrack_kernel(const double *__restrict__ cost,
+                                                                  const double *__restrict__ tab, int num_part, int64_t n,
+                                                                  int64_t *__restrict__ upper) {
+    __shared__ double s_v[8];
+    __shared__ int64_t s_i[8];
+    __shared__ int64_t s_u;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int64_t u = n - 1;
+    if (threadIdx.x == 0) upper[num_part - 1] = u;
+    for (int p = num_part; p >= 2; --p) {
+        const double *prev = tab + (int64_t)((p == num_part ? p - 1 : p) - 1) * n;
+        const double *col = cost + u * (u + 1) / 2 + 1;
+        double bv = (double)INFINITY;
+        int64_t bi = INT64_MAX;
+        for (int64_t u1 = p - 2 + threadIdx.x; u1 < u; u1 += blockDim.x) {
+            const double v = __dadd_rn(prev[u1], col[u1]);
+            if (v < bv) { bv = v; bi = u1; }   // ascending in each thread: the strict test keeps the first
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1)
+            argmin_first(bv, bi, __shfl_xor_sync(0xFFFFFFFFu, bv, o), __shfl_xor_sync(0xFFFFFFFFu, bi, o));
+        if (lane == 0) { s_v[warp] = bv; s_i[warp] = bi; }
+        __syncthreads();
+        if (warp == 0) {
+            const int nw = (int)(blockDim.x >> 5);
+            bv = lane < nw ? s_v[lane] : (double)INFINITY;
+            bi = lane < nw ? s_i[lane] : INT64_MAX;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1)
+                argmin_first(bv, bi, __shfl_xor_sync(0xFFFFFFFFu, bv, o), __shfl_xor_sync(0xFFFFFFFFu, bi, o));
+            if (lane == 0) { upper[p - 2] = bi; s_u = bi; }
+        }
+        __syncthreads();
+        u = s_u;
+    }
+}
+
+bool partition_terms_in_smem(int64_t n) { return n <= kPartitionSmemTerms; }
+int64_t partition_term_rows(int64_t n) { return partition_terms_in_smem(n) ? 0 : (n < kPartitionTermRows ? n : kPartitionTermRows); }
+
+// The triangle into cost; with tab != nullptr (2 <= num_part < n) also the tables (num_part - 1 rows of n) and the upper
+// index of each partition into upper[num_part].  g_terms: partition_term_rows(n) rows of n doubles (or nullptr if 0).
+cudaError_t ensemble_partition(const int64_t *sizes, const int64_t *counts, int64_t n, int num_part, double *cost, double *tab,
+                               double *g_terms, int64_t *upper, int sm_count, cudaStream_t s) {
+    cudaError_t e;
+    if (partition_terms_in_smem(n)) {
+        const int smem = (int)(n * 8);
+        e = cudaFuncSetAttribute(partition_cost_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        if (e != cudaSuccess) return e;
+        DSK_LAUNCH(partition_cost_kernel<true>, (unsigned)n, kPartitionCostThreads, (size_t)smem, s, sizes, counts, n, cost,
+                   tab, nullptr);
+    } else {
+        DSK_LAUNCH(partition_cost_kernel<false>, (unsigned)partition_term_rows(n), kPartitionCostThreads, 0, s, sizes, counts,
+                   n, cost, tab, g_terms);
+    }
+    e = cudaGetLastError();
+    if (e != cudaSuccess || !tab) return e;
+    if (num_part > 2) e = cudaMemsetAsync(tab + n, 0, (size_t)(num_part - 2) * n * 8, s);
+    int64_t g = (n + 7) / 8;
+    if (g > (int64_t)sm_count * 16) g = (int64_t)sm_count * 16;
+    for (int p = 2; p < num_part && e == cudaSuccess; ++p) {
+        DSK_LAUNCH(partition_dp_kernel, (unsigned)g, 256, 0, s, (const double *)cost, (const double *)(tab + (int64_t)(p - 2) * n),
+                   tab + (int64_t)(p - 1) * n, p, n);
+        e = cudaGetLastError();
+    }
+    if (e != cudaSuccess) return e;
+    DSK_LAUNCH(partition_backtrack_kernel, 1, 256, 0, s, (const double *)cost, (const double *)tab, num_part, n, upper);
+    return cudaGetLastError();
+}
+
+}  // namespace dsk

@@ -3,9 +3,12 @@ datasketch/lshensemble_partition.py), on top of this package's ``MinHashLSH``.
 
 What runs where:
 
-* parameter tables (``_optimal_param``: scipy ``quad`` over ten x/q ratios) and the size partitioner
-  (``optimal_partitions``: dynamic programme over the distinct set sizes) are host-side control logic, float64,
-  the same expressions in the same order as the reference so the chosen (b, r) and partition bounds are identical;
+* parameter tables (``_optimal_param``: scipy ``quad`` over ten x/q ratios) are host-side control logic, float64, the
+  same expressions in the same order as the reference so the chosen (b, r) are identical;
+* the size partitioner (dynamic programme over the distinct set sizes) has two implementations with the reference's
+  bounds: ``optimal_partitions`` on the host (``MinHashLSHEnsemble``, and the tests' reference) and
+  ``optimal_partitions_device``, whose cost table (cubic in the number of distinct sizes), dynamic programme and
+  back-tracking run on the device (``dsk_ensemble_partition``; ``GpuLSHEnsemble.index`` uses it);
 * ``index`` inserts each partition's sets into its ``MinHashLSH`` instances with ``insert_batch``: the band keys of
   the whole partition come from one ``dsk_band_keys`` launch per distinct r instead of one ``_H`` call per set
   and band (lshensemble.py:221-228 -> lsh.py:344);
@@ -118,6 +121,54 @@ def optimal_partitions(sizes, counts, num_part: int) -> List[Tuple[int, int]]:
         p -= 1
     bounds.insert(0, (sizes[0], sizes[u]))
     return bounds
+
+
+def optimal_partitions_device(sizes, counts, num_part: int, device: int = 0) -> List[Tuple[int, int]]:
+    """``optimal_partitions(sizes, counts, num_part)``, the same list of ``(lower, upper)`` tuples of the input's sizes, with
+    the interval costs, the dynamic programme and the back-tracking on CUDA device ``device`` (``dsk_ensemble_partition``).
+
+    ``sizes`` (strictly ascending, > 0) and ``counts`` (> 0) are integer sequences of one length D >= 1, each value below
+    2^62; ``ValueError`` otherwise.  Every cost is the reference's float64 value bit for bit (its numpy pairwise sums
+    included) and every argmin takes the first index among equal values, so the bounds are the reference's.  The
+    workspace, about ``4 * D * (D + 1) + 8 * D * num_part`` bytes of device memory (``dsk_ensemble_partition_workspace_size``),
+    is allocated with torch; ``MemoryError`` names D and the bytes if it cannot be.  ``num_part < 2`` and ``num_part >= D``
+    need no table and are answered on the host, as in ``optimal_partitions``."""
+    from . import _native as nv
+    sz = np.asarray(sizes)
+    ct = np.asarray(counts)
+    if sz.ndim != 1 or ct.ndim != 1 or len(sz) != len(ct) or len(sz) == 0:
+        raise ValueError("sizes and counts must be 1-D sequences of one length >= 1 (got %s and %s)" % (sz.shape, ct.shape))
+    if sz.dtype.kind not in "iu" or ct.dtype.kind not in "iu":
+        raise TypeError("set sizes and counts must be integers")
+    if np.any(sz < 0) or np.any(ct < 0):   # a negative value would wrap in a uint64 -> int64 cast; the C-ABI names it
+        raise ValueError("set sizes and counts must be positive")
+    s64 = np.ascontiguousarray(sz, dtype=np.int64)
+    c64 = np.ascontiguousarray(ct, dtype=np.int64)
+    n = len(s64)
+    lib = nv.load()
+    out = np.zeros(max(min(num_part, n), 1), dtype=np.int64)
+    if num_part < 2 or num_part >= n:   # no table: the C-ABI only checks the input and writes the trivial bounds
+        nv.check(lib.dsk_ensemble_partition(s64.ctypes.data, c64.ctypes.data, n, num_part, None, 0, device,
+                                            out.ctypes.data, None, None))
+    else:
+        import torch
+        nv.require_device(device)
+        need = int(lib.dsk_ensemble_partition_workspace_size(n, num_part))
+        try:
+            ws = torch.empty((need,), dtype=torch.uint8, device="cuda:%d" % device)
+        except torch.OutOfMemoryError as exc:
+            raise MemoryError("optimal_partitions_device: cannot allocate the %d bytes of device memory the partitioner "
+                              "needs for D = %d distinct set sizes and num_part = %d" % (need, n, num_part)) from exc
+        with torch.cuda.device(device):
+            nv.check(lib.dsk_ensemble_partition(s64.ctypes.data, c64.ctypes.data, n, num_part, ws.data_ptr(), need, device,
+                                                out.ctypes.data, None, torch.cuda.current_stream().cuda_stream))
+        del ws
+    if num_part < 2:
+        return [(sz[0], sz[-1])]
+    if num_part >= n:
+        return [(x, x) for x in sz]
+    lowers = np.concatenate([[0], out[:-1] + 1])
+    return [(sz[lo], sz[up]) for lo, up in zip(lowers.tolist(), out.tolist())]
 
 
 # ---- the index ------------------------------------------------------------------------------------------------
@@ -252,14 +303,15 @@ def _partition_ranges(sorted_sizes: np.ndarray, uppers: list) -> np.ndarray:
     return start
 
 
-def _index_plan(sizes: np.ndarray, num_part: int):
-    """Host side of ``GpuLSHEnsemble.index`` for set sizes ``int64[N]``: ``(lowers, uppers, order, start)`` -- the
-    reference's partition bounds over ``Counter(sizes)`` (None for the unused trailing partitions), the stable size order
-    (``order[t]`` = the row that becomes set number t, as ``entries.sort(key=size)``) and the partitions as ranges of
-    set numbers."""
+def _index_plan(sizes: np.ndarray, num_part: int, partitioner=optimal_partitions):
+    """Plan of ``GpuLSHEnsemble.index`` for set sizes ``int64[N]``: ``(lowers, uppers, order, start)`` -- the
+    reference's partition bounds over ``Counter(sizes)`` (None for the unused trailing partitions) from ``partitioner``
+    (``optimal_partitions`` or a function with its contract, such as ``optimal_partitions_device`` bound to a device),
+    the stable size order (``order[t]`` = the row that becomes set number t, as ``entries.sort(key=size)``) and the
+    partitions as ranges of set numbers."""
     vals, counts = np.unique(sizes, return_counts=True)      # = sorted(Counter(sizes).most_common())
     lowers, uppers = [None] * num_part, [None] * num_part
-    for i, (lower, upper) in enumerate(optimal_partitions(vals, counts, num_part)):
+    for i, (lower, upper) in enumerate(partitioner(vals, counts, num_part)):
         lowers[i], uppers[i] = lower, upper
     order = np.argsort(sizes, kind="stable")
     return lowers, uppers, order, _partition_ranges(sizes[order], uppers)
@@ -385,7 +437,8 @@ class GpuLSHEnsemble:
                 raise ValueError("keys must hold one key per row of sig (%d), got %d" % (n, len(keys)))
         if n >= 1 << 31:
             raise ValueError("an index holds fewer than 2^31 sets")
-        lowers, uppers, order, start = _index_plan(sizes, self.num_part)
+        lowers, uppers, order, start = _index_plan(
+            sizes, self.num_part, lambda s, c, k: optimal_partitions_device(s, c, k, device=self.device))
         d_order = torch.from_numpy(order.astype(np.int32)).to(d_sig.device)
         with torch.cuda.device(self.device):
             nv.check(nv.load().dsk_lsh_ensemble_index(self._h, d_sig.data_ptr(), n, d_order.data_ptr(), start.ctypes.data,

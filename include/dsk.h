@@ -391,6 +391,34 @@ DSK_API int dsk_lsh_ensemble_query_count(const dsk_lsh_ensemble *e, const uint32
                                          int64_t *d_counts, void *stream);
 DSK_API int dsk_lsh_ensemble_query_fill(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int32_t *d_sel,
                                         const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq, void *stream);
+/* The size partitions of MinHashLSHEnsemble.index (lshensemble_partition.py:54-196, optimal_partitions), on the device.
+ * h_sizes / h_counts (host memory, n_sizes = D entries): the distinct set sizes, strictly ascending, and their counts, every
+ * value in [1, 2^62).  Writes h_upper_idx[k] (host memory, min(num_part, D) entries) = the index into h_sizes of the upper
+ * bound of partition k; partition k covers sizes (h_upper_idx[k-1], h_upper_idx[k]] (from index 0 for k = 0), the last ends
+ * at D - 1.  These are the reference's bounds bit for bit: cost[l, u] = sum over i in [l, u] of (sizes[u] - sizes[i]) /
+ * sizes[u] * counts[i] with each operation rounded on its own and numpy's float64 pairwise summation, the reference's
+ * dynamic programme (its back-tracking reads the p-interval table where the recurrence used p - 1, reproduced), and every
+ * argmin takes the first index among equal values.
+ *   dsk_ensemble_partition_workspace_size  bytes of d_workspace (16-byte aligned), each part rounded up to 256 bytes:
+ *                        16 * D (sizes, counts); for D > 28672 also 8 * D * min(D, 512) (terms of the cost columns, which
+ *                        fit shared memory below); for 2 <= num_part < D also 4 * D * (D + 1) (the cost triangle, 50 MB at
+ *                        D = 3550, 1.6 GB at D = 20000) + 8 * D * (num_part - 1) (the tables) + 8 * num_part.  0 for
+ *                        n_sizes < 1 or num_part < 1; SIZE_MAX if the sum does not fit in size_t.
+ *   dsk_ensemble_partition  num_part < 2 (one partition) and num_part >= D (one per size) need no table: the bounds are
+ *                        written on the host, with no device work and no workspace, unless d_cost is given.  Otherwise it
+ *                        copies sizes and counts to the device, fills the triangle, runs num_part - 2 launches of the
+ *                        programme and one of the back-tracking, copies the num_part indices back and synchronises the
+ *                        stream once, at the end.  d_cost (may be NULL; device memory, D(D+1)/2 doubles): the triangle is
+ *                        written there instead of the workspace, entry (l, u) at u(u+1)/2 + l, in every case.
+ *                        DSK_ERR_INVALID (with a message) for n_sizes < 1, num_part < 1, null host buffers, sizes not
+ *                        strictly ascending or outside [1, 2^62), counts outside [1, 2^62), and a workspace that is too
+ *                        small or not 16-byte aligned.
+ * Cost: D^3/6 float64 additions and D^2/2 divisions for the triangle (one CTA per column, one thread per entry, the column's
+ * terms shared), then num_part reads of it. */
+DSK_API size_t dsk_ensemble_partition_workspace_size(int64_t n_sizes, int num_part);
+DSK_API int dsk_ensemble_partition(const int64_t *h_sizes, const int64_t *h_counts, int64_t n_sizes, int num_part,
+                                   void *d_workspace, size_t workspace_bytes, int device, int64_t *h_upper_idx,
+                                   double *d_cost, void *stream);
 DSK_API int dsk_lsh_remove(dsk_lsh *ix, const int32_t *d_docs, int64_t n, int64_t *d_status, void *stream);
 DSK_API int dsk_lsh_alive(const dsk_lsh *ix, const int32_t *d_docs, int64_t n, uint8_t *d_out, void *stream);
 DSK_API size_t dsk_lsh_compact_workspace_size(const dsk_lsh *ix);
