@@ -105,6 +105,9 @@ SIGNATURES = {
                                  c_void_p]),
     "dsk_bloom_query": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, ctypes.c_uint64, ctypes.c_uint64, c_int,
                                 c_void_p, c_void_p]),
+    "dsk_bloom_unique_workspace_size": (c_size_t, [c_int64, c_int, c_int, c_int, c_int]),
+    "dsk_bloom_unique": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, ctypes.c_uint64, ctypes.c_uint64, c_int,
+                                 c_void_p, c_size_t, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -600,6 +600,57 @@ int dsk_bloom_query(const uint32_t *d_sig, int64_t n, int num_perm, int b, int r
     return DSK_OK;
 }
 
+// the n * b * n_hashes probe entries of a batch are numbered in int32: at most kBloomUniqueMaxEntries (checked without
+// overflow: b and n_hashes are positive ints, so b * n_hashes fits int64)
+static bool bloom_unique_fits(int64_t n, int b, int n_hashes) {
+    return n <= kBloomUniqueMaxEntries / ((int64_t)b * n_hashes);
+}
+
+size_t dsk_bloom_unique_workspace_size(int64_t n, int num_perm, int b, int r, int n_hashes) {
+    if (n <= 0 || num_perm <= 0 || b <= 0 || r <= 0 || (int64_t)b * r > num_perm || n_hashes <= 0 || n_hashes > 64 ||
+        !bloom_unique_fits(n, b, n_hashes))
+        return 0;
+    return bloom_unique_workspace_bytes(n, b, n_hashes);
+}
+
+int dsk_bloom_unique(const uint32_t *d_sig, int64_t n, int num_perm, int b, int r, uint32_t *d_bits, uint64_t words_per_table,
+                     uint64_t n_bits, int n_hashes, void *d_ws, size_t ws_bytes, uint8_t *d_keep, void *stream) {
+    const char *who = "dsk_bloom_unique";
+    int rc = check_bands(who, n, num_perm, b, r);
+    if (rc) return rc;
+    rc = check_bloom(who, d_bits, words_per_table, n_bits, n_hashes);
+    if (rc) return rc;
+    if (n_bits > (UINT64_MAX - 1) / (uint64_t)b) {   // the batch table's key band * n_bits + pos must not reach the empty key
+        set_error("%s: b * n_bits must be below 2^64 (got b=%d n_bits=%llu)", who, b, (unsigned long long)n_bits);
+        return DSK_ERR_INVALID;
+    }
+    if (n == 0) return DSK_OK;
+    if (!d_sig || !d_ws || !d_keep) {
+        set_error("%s: null buffer", who);
+        return DSK_ERR_INVALID;
+    }
+    if (((uintptr_t)d_sig & 3) != 0 || ((uintptr_t)d_ws & 15) != 0) {
+        set_error("%s: d_sig must be 4-byte and d_ws 16-byte aligned", who);
+        return DSK_ERR_ALIGN;
+    }
+    if (!bloom_unique_fits(n, b, n_hashes)) {
+        set_error("%s: n * b * n_hashes must be at most 2^30 (got n=%lld b=%d n_hashes=%d); split the batch", who,
+                  (long long)n, b, n_hashes);
+        return DSK_ERR_INVALID;
+    }
+    const size_t need = bloom_unique_workspace_bytes(n, b, n_hashes);
+    if (ws_bytes < need) {
+        set_error("%s: the workspace must hold dsk_bloom_unique_workspace_size() = %zu bytes (got %zu)", who, need, ws_bytes);
+        return DSK_ERR_INVALID;
+    }
+    DevInfo *dev;
+    rc = current_dev(&dev);
+    if (rc) return rc;
+    DSK_CUDA(bloom_unique(d_sig, n, num_perm, b, r, d_bits, words_per_table, n_bits, n_hashes, d_ws, d_keep, dev->sm_count,
+                          (cudaStream_t)stream));
+    return DSK_OK;
+}
+
 int dsk_wmh_create(const float *h_rs, const float *h_ln_cs, const float *h_betas, int sample_size, int dim, int device,
                    dsk_wmh **out) {
     if (!h_rs || !h_ln_cs || !h_betas || !out || sample_size <= 0 || dim <= 0) {

@@ -25,6 +25,7 @@ static inline double __dsub_rn(double a, double b) { return a - b; }
 static inline double __dmul_rn(double a, double b) { return a * b; }
 static inline double __ddiv_rn(double a, double b) { return a / b; }
 static inline double __ll2double_rn(long long v) { return (double)v; }
+static inline uint64_t __umul64hi(uint64_t a, uint64_t b) { return (uint64_t)(((unsigned __int128)a * b) >> 64); }
 #else
 #define DSK_LAUNCH(kernel, grid, block, smem, stream, ...) kernel<<<grid, block, smem, stream>>>(__VA_ARGS__)
 #define DSK_DYNAMIC_SMEM(name) extern __shared__ __align__(128) unsigned char name[]
@@ -110,6 +111,13 @@ cudaError_t launch_bloom_insert(const uint32_t *sig, int64_t n, int k, int b, in
 cudaError_t launch_bloom_query(const uint32_t *sig, int64_t n, int k, int b, int r, const uint32_t *bits,
                                uint64_t words_per_table, uint64_t n_bits, int n_hashes, uint8_t *hit, int sm_count,
                                cudaStream_t s);
+// insert_unique of a batch of n rows (DESIGN.md §4i): the workspace, and the probe / resolve / commit stages writing keep[n],
+// with no host synchronisation.  Entries (one per probe bit not set before the call) are numbered in int32 and their slots
+// too, so a call takes at most kBloomUniqueMaxEntries = n * b * n_hashes.
+constexpr int64_t kBloomUniqueMaxEntries = (int64_t)1 << 30;
+size_t bloom_unique_workspace_bytes(int64_t n, int b, int n_hashes);
+cudaError_t bloom_unique(const uint32_t *sig, int64_t n, int k, int b, int r, uint32_t *bits, uint64_t words_per_table,
+                         uint64_t n_bits, int n_hashes, void *ws, uint8_t *keep, int sm_count, cudaStream_t s);
 
 cudaError_t launch_wmh_transpose(const float *src, int ss, int dim, int ss_pad, float *dst, cudaStream_t s);
 cudaError_t launch_wmh(const float *rs_t, const float *lncs_t, const float *betas_t, int ss, int ss_pad, int dim,
@@ -303,6 +311,66 @@ __device__ __forceinline__ uint64_t band_fp(const uint32_t *v, int r, int band) 
     for (int q = 0; q < r; ++q) h = (h ^ v[q]) * 0xFF51AFD7ED558CCDull + 0x2545F4914F6CDD1Dull;
     h = lsh_mix64(h);
     return h == kEmptyKey ? h - 1 : h;
+}
+
+// ---- relaxed loads and stores (union-find parents, insert_unique's statuses) ----------------------------------------------
+// Loads and stores of values that race with other threads' writes: relaxed, so a racing reader sees an old or a new value.
+// The CPU emulation (-DDSK_EMU) uses the same relaxed atomics of GCC, so ThreadSanitizer checks every other access.
+#ifdef DSK_EMU
+inline int32_t ld_relaxed(const int32_t *p) { return __atomic_load_n(p, __ATOMIC_RELAXED); }
+inline void st_relaxed(int32_t *p, int32_t v) { __atomic_store_n(p, v, __ATOMIC_RELAXED); }
+#else
+__device__ __forceinline__ int32_t ld_relaxed(const int32_t *p) {
+    int32_t v;
+    asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_relaxed(int32_t *p, int32_t v) {
+    asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+#endif
+
+// ---- the greedy resolution of insert_unique (GpuLSH: lsh_kernels.cu, DESIGN.md §4e; MinHashLSHBloom: bloom_kernels.cu,
+// §4i) ---------------------------------------------------------------------------------------------------------------------
+// Statuses go UNDECIDED -> KEPT / DROPPED.  `decide(j)` decides row j from the FINAL statuses of the rows before it and
+// writes st[j] with st_relaxed, or returns false (row j waits).  Whichever order rows are visited in and whichever of the
+// other threads' writes of a round a visit sees, every decision is the serial loop's; the smallest undecided row can always
+// decide, so every round decides at least one row.
+enum : int32_t { kUndecided = 0, kKept = 1, kDropped = 2 };
+constexpr int kUniqueSweeps = 3;           // grid-wide rounds before the remainder goes to one CTA
+constexpr int kResolveThreads = 1024;      // the CTA that finishes the rounds
+
+// one grid-wide round over every undecided row; list != nullptr: appends the rows that stay undecided (in any order)
+template <class Decide>
+__device__ __forceinline__ void unique_sweep(const Decide &decide, const int32_t *st, int64_t n, int32_t *list,
+                                             unsigned *list_n) {
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+        if (ld_relaxed(st + j) != kUndecided) continue;
+        if (!decide(j) && list) list[atomicAdd(list_n, 1u)] = (int32_t)j;
+    }
+}
+
+// ONE CTA: rounds over the listed rows until every row is decided; each round lists its still undecided rows in the other
+// buffer.  Every round decides at least the smallest listed row, so the loop ends.
+template <class Decide>
+__device__ __forceinline__ void unique_resolve(const Decide &decide, int32_t *list, int32_t *spare, const unsigned *list_n) {
+    __shared__ unsigned s_left;
+    unsigned left = *list_n;
+    int32_t *cur = list, *nxt = spare;
+    while (left > 0) {
+        __syncthreads();   // every thread has read s_left before it is reset
+        if (threadIdx.x == 0) s_left = 0;
+        __syncthreads();
+        for (unsigned i = threadIdx.x; i < left; i += blockDim.x) {
+            const int32_t j = cur[i];
+            if (!decide(j)) nxt[atomicAdd(&s_left, 1u)] = j;
+        }
+        __syncthreads();
+        left = s_left;
+        int32_t *t = cur;
+        cur = nxt;
+        nxt = t;
+    }
 }
 
 }  // namespace dsk

@@ -315,21 +315,7 @@ cudaError_t launch_forest_query(const uint32_t *sig, const int32_t *order, int64
 // smallest document number.
 namespace dsk {
 
-// Loads and stores of union-find parents that race with hooks: relaxed, so a racing reader sees an old or a new parent.
-// The CPU emulation (-DDSK_EMU) uses the same relaxed atomics of GCC, so ThreadSanitizer checks every other access.
-#ifdef DSK_EMU
-inline int32_t ld_relaxed(const int32_t *p) { return __atomic_load_n(p, __ATOMIC_RELAXED); }
-inline void st_relaxed(int32_t *p, int32_t v) { __atomic_store_n(p, v, __ATOMIC_RELAXED); }
-#else
-__device__ __forceinline__ int32_t ld_relaxed(const int32_t *p) {
-    int32_t v;
-    asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_relaxed(int32_t *p, int32_t v) {
-    asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-#endif
+// Loads and stores of union-find parents that race with hooks are relaxed (ld_relaxed / st_relaxed, dsk_common.cuh).
 
 // Lock-free union-find on parent[] with parent[x] <= x at all times.  A hook replaces a root's self-link by a SMALLER
 // root (atomicCAS, so it fails if the root was hooked meanwhile), so every path strictly decreases and the root of each
@@ -912,12 +898,9 @@ cudaError_t lsh_compact(const LshDev &ix, const uint32_t *removed, int64_t n_doc
 // always decide, so every round decides at least one row; a drift chain (row j's only partner is j - 1) of length L takes
 // about L rounds.  The rounds run as kUniqueSweeps grid-wide sweeps (one launch each, no host synchronisation), the last
 // of which lists the rows still undecided; one CTA then loops over that list, round after round, separated by
-// __syncthreads, until it is empty.  No CTA ever waits for another.
+// __syncthreads, until it is empty.  No CTA ever waits for another.  The statuses and both schedules (unique_sweep,
+// unique_resolve) are dsk_common.cuh's, shared with MinHashLSHBloom's insert_unique.
 namespace dsk {
-
-enum : int32_t { kUndecided = 0, kKept = 1, kDropped = 2 };
-constexpr int kUniqueSweeps = 3;           // grid-wide rounds before the remainder goes to one CTA
-constexpr int kResolveThreads = 1024;      // the CTA that finishes the rounds
 
 // Decides row j from the statuses of its earlier partners pidx[ptr[j] .. ptr[j + 1]); false: j stays undecided.
 __device__ __forceinline__ bool unique_decide(const int64_t *ptr, const int32_t *pidx, int32_t *st, int64_t j) {
@@ -944,35 +927,14 @@ __global__ void __launch_bounds__(256) unique_init_kernel(const int32_t *__restr
 // one grid-wide round over every undecided row; list != nullptr: appends the rows that stay undecided (in any order)
 __global__ void __launch_bounds__(256) unique_sweep_kernel(const int64_t *__restrict__ ptr, const int32_t *__restrict__ pidx,
                                                            int32_t *st, int64_t n, int32_t *list, unsigned *list_n) {
-    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
-        if (ld_relaxed(st + j) != kUndecided) continue;
-        if (!unique_decide(ptr, pidx, st, j) && list) list[atomicAdd(list_n, 1u)] = (int32_t)j;
-    }
+    unique_sweep([&](int64_t j) { return unique_decide(ptr, pidx, st, j); }, st, n, list, list_n);
 }
 
-// ONE CTA: rounds over the listed rows until every row is decided; each round lists its still undecided rows in the other
-// buffer.  Every round decides at least the smallest listed row, so the loop ends.
 __global__ void __launch_bounds__(kResolveThreads) unique_resolve_kernel(const int64_t *__restrict__ ptr,
                                                                          const int32_t *__restrict__ pidx, int32_t *st,
                                                                          int32_t *list, int32_t *spare,
                                                                          const unsigned *list_n) {
-    __shared__ unsigned s_left;
-    unsigned left = *list_n;
-    int32_t *cur = list, *nxt = spare;
-    while (left > 0) {
-        __syncthreads();   // every thread has read s_left before it is reset
-        if (threadIdx.x == 0) s_left = 0;
-        __syncthreads();
-        for (unsigned i = threadIdx.x; i < left; i += blockDim.x) {
-            const int32_t j = cur[i];
-            if (!unique_decide(ptr, pidx, st, j)) nxt[atomicAdd(&s_left, 1u)] = j;
-        }
-        __syncthreads();
-        left = s_left;
-        int32_t *t = cur;
-        cur = nxt;
-        nxt = t;
-    }
+    unique_resolve([&](int64_t j) { return unique_decide(ptr, pidx, st, j); }, list, spare, list_n);
 }
 
 // flags[j] = 1 for a kept row (the exclusive scan of the flags numbers the kept rows), kept[j] the caller's copy

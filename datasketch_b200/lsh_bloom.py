@@ -106,7 +106,8 @@ def band_keys_host(hashvalues: np.ndarray, b: int, r: int) -> np.ndarray:
 class MinHashLSHBloom:
     """Drop-in for ``datasketch.MinHashLSHBloom`` (lsh_bloom.py:125): ``insert(minhash)``, ``query(minhash) -> bool``,
     ``sync()``, ``hashtables`` (one ``BloomTable`` per band); plus ``insert_batch(signatures)`` /
-    ``query_batch(signatures) -> bool array`` on [N, K] matrices (one kernel launch each)."""
+    ``query_batch(signatures) -> bool array`` on [N, K] matrices (one kernel launch each), and
+    ``insert_unique(signatures) -> keep``, the query-then-insert de-duplication loop over a whole matrix."""
 
     def __init__(self, threshold: float = 0.9, num_perm: int = 128, n: Optional[int] = None, fp: Optional[float] = None,
                  save_dir: Optional[str] = None, weights: Tuple[float, float] = (0.5, 0.5),
@@ -186,6 +187,46 @@ class MinHashLSHBloom:
                                                self._bits.data_ptr(), self.words_per_table, self.n_bits, self.n_hashes,
                                                hit.data_ptr(), torch.cuda.current_stream().cuda_stream))
         return hit.cpu().numpy().astype(bool) if to_host else hit.bool()
+
+    def insert_unique(self, signatures, to_host: bool = True):
+        """The streaming de-duplication loop over a whole [N, K] signature matrix, on the device::
+
+            for m in rows:
+                if not self.query(m):
+                    self.insert(m)
+
+        Returns ``keep``: ``keep[j]`` is True iff that loop, run over the rows in order from the tables as they are at
+        the call, inserts row j.  The tables afterwards hold exactly the bits the loop leaves, i.e. their bits before
+        the call plus ``insert_batch(signatures[keep])``.  Bloom false positives count exactly as the loop meets them:
+        a band is covered when each of its probe bits is set, before the call or by kept rows earlier in the batch.
+        ``query_batch`` followed by ``insert_batch`` of the misses is not the same: it keeps both rows of a
+        near-duplicate pair inside one batch.
+
+        Input as ``insert_batch``.  Stream-ordered with no host synchronisation (``to_host=False`` returns a CUDA bool
+        tensor).  The workspace, about ``32 * b * n_hashes + 12`` bytes per row (``dsk_bloom_unique_workspace_size``),
+        is allocated with torch; ``MemoryError`` names N and the bytes if it cannot be.  Batches of more than
+        ``2^30 / (b * n_hashes)`` rows run as consecutive calls over slices, which give the same result."""
+        import torch
+        d_sig = self._dev_sig(signatures)
+        n = d_sig.shape[0]
+        keep = torch.empty((n,), dtype=torch.uint8, device=d_sig.device)
+        lib = nv.load()
+        step = max(1, (1 << 30) // (self.b * self.n_hashes))
+        if n:
+            need = int(lib.dsk_bloom_unique_workspace_size(min(n, step), self.h, self.b, self.r, self.n_hashes))
+            try:
+                ws = torch.empty((need,), dtype=torch.uint8, device=d_sig.device)
+            except torch.OutOfMemoryError as exc:
+                raise MemoryError("MinHashLSHBloom.insert_unique: cannot allocate the %d bytes of device memory the "
+                                  "workspace needs for N = %d rows" % (need, min(n, step))) from exc
+            with torch.cuda.device(self.device):
+                stream = torch.cuda.current_stream().cuda_stream
+                for lo in range(0, n, step):
+                    rows = d_sig[lo:lo + step]
+                    nv.check(lib.dsk_bloom_unique(rows.data_ptr(), rows.shape[0], self.h, self.b, self.r,
+                                                  self._bits.data_ptr(), self.words_per_table, self.n_bits, self.n_hashes,
+                                                  ws.data_ptr(), need, keep[lo:].data_ptr(), stream))
+        return keep.cpu().numpy().astype(bool) if to_host else keep.bool()
 
     # ---- the reference's single-object API -------------------------------------------------------------------
     def _row(self, minhash) -> np.ndarray:

@@ -182,6 +182,18 @@ DSK_API int dsk_bloom_insert(const uint32_t *d_sig, int64_t n, int num_perm, int
                              uint64_t words_per_table, uint64_t n_bits, int n_hashes, void *stream);
 DSK_API int dsk_bloom_query(const uint32_t *d_sig, int64_t n, int num_perm, int b, int r, const uint32_t *d_bits,
                             uint64_t words_per_table, uint64_t n_bits, int n_hashes, uint8_t *d_hit, void *stream);
+/* dsk_bloom_unique: the loop `for each row j in order: if not query(row j): insert(row j)` over a whole batch, on the
+ * device.  d_keep[j] = 1 iff the loop inserts row j, and d_bits afterwards hold exactly the bits the loop leaves (the
+ * prior bits plus dsk_bloom_insert of the kept rows), Bloom false positives included.  Stream-ordered, no host
+ * synchronisation.  d_sig 4-byte aligned; d_ws 16-byte aligned and at least dsk_bloom_unique_workspace_size() bytes:
+ * with E = n * b * n_hashes probe entries, 24*E (key table at load factor 1/2) + 8*E (entry slots and links) + 12*n
+ * bytes, each of its 8 parts rounded up to 256.  The workspace size is 0 for n <= 0, for invalid (num_perm, b, r,
+ * n_hashes) and for E > 2^30, which dsk_bloom_unique rejects (split the batch: consecutive calls give the same result as
+ * one call over their concatenation).  n_bits must satisfy b * n_bits < 2^64. */
+DSK_API size_t dsk_bloom_unique_workspace_size(int64_t n, int num_perm, int b, int r, int n_hashes);
+DSK_API int dsk_bloom_unique(const uint32_t *d_sig, int64_t n, int num_perm, int b, int r, uint32_t *d_bits,
+                             uint64_t words_per_table, uint64_t n_bits, int n_hashes, void *d_ws, size_t ws_bytes,
+                             uint8_t *d_keep, void *stream);
 
 /* ---- Weighted MinHash (Ioffe ICWS) ------------------------------------------------------
  * Handle = device copy of the generator parameters rs, ln_cs, betas, each [sample_size, dim]
