@@ -96,6 +96,12 @@ SIGNATURES = {
     "dsk_bbit_unpack": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),
     "dsk_forest_query": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_int, c_void_p,
                                  c_void_p]),
+    "dsk_forest_query_weighted": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_int,
+                                          c_void_p, c_void_p]),
+    "dsk_forest_query_topk": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_int,
+                                      c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "dsk_forest_neighbors": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                     c_void_p, c_void_p, c_void_p]),
     "dsk_lean_pack": (c_int, [c_void_p, c_int, c_int64, c_int, c_int64, c_int, c_void_p, c_void_p]),
     "dsk_lean_unpack": (c_int, [c_void_p, c_int64, c_int, c_int64, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "dsk_band_keys": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p]),

@@ -1680,6 +1680,75 @@ int dsk_forest_query(const uint32_t *d_sig, const int32_t *d_order, int64_t n, i
     return DSK_OK;
 }
 
+// The ranked and weighted forest walks.  num_perm, l and k count samples (weighted rows are [n, 2 * num_perm] words).
+static int check_forest(const char *who, const uint32_t *d_sig, const int32_t *d_order, int64_t n, int num_perm, int weighted,
+                        int l, int k, const uint32_t *d_qsig, int64_t nq) {
+    if (n < 0 || nq < 0 || num_perm <= 0 || num_perm > (1 << 29) || l <= 0 || k <= 0 || (int64_t)l * k > num_perm ||
+        (weighted != 0 && weighted != 1) || (n > 0 && (!d_sig || !d_order)) || (nq > 0 && !d_qsig)) {
+        set_error("%s: bad arguments (need 0 < l*k <= num_perm, weighted 0 or 1, buffers where work exists)", who);
+        return DSK_ERR_INVALID;
+    }
+    if (weighted && ((n > 0 && ((uintptr_t)d_sig & 7) != 0) || (nq > 0 && ((uintptr_t)d_qsig & 7) != 0))) {
+        set_error("%s: weighted rows must be 8-byte aligned", who);
+        return DSK_ERR_INVALID;
+    }
+    return DSK_OK;
+}
+
+static int check_forest_topk(const char *who, int num_perm, int candidates, int min_count, int topk, int64_t rows,
+                             const int32_t *d_idx, const int32_t *d_eq) {
+    if (topk < 1 || topk > 32 || candidates < topk || candidates > 1024 || min_count < 0 || min_count > num_perm ||
+        (rows > 0 && (!d_idx || !d_eq))) {
+        set_error("%s: bad arguments (need 1 <= topk <= 32, topk <= candidates <= 1024, 0 <= min_count <= num_perm, "
+                  "output buffers)", who);
+        return DSK_ERR_INVALID;
+    }
+    return DSK_OK;
+}
+
+int dsk_forest_query_weighted(const uint32_t *d_sig, const int32_t *d_order, int64_t n, int sample_size, int l, int k,
+                              const uint32_t *d_qsig, int64_t nq, int topk, int32_t *d_out, void *stream) {
+    int rc = check_forest("dsk_forest_query_weighted", d_sig, d_order, n, sample_size, 1, l, k, d_qsig, nq);
+    if (rc) return rc;
+    if (topk <= 0 || topk > 1024 || (nq > 0 && !d_out)) {
+        set_error("dsk_forest_query_weighted: bad arguments (need 0 < topk <= 1024, an output buffer)");
+        return DSK_ERR_INVALID;
+    }
+    DevInfo *dev;
+    rc = current_dev(&dev);
+    if (rc) return rc;
+    DSK_CUDA(launch_forest(FOREST_SET, 2, d_sig, d_order, n, 2 * sample_size, l, k, d_qsig, nq, topk, d_out, nullptr, 0, 0,
+                           dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_forest_query_topk(const uint32_t *d_sig, const int32_t *d_order, int64_t n, int num_perm, int weighted, int l,
+                          int k, const uint32_t *d_qsig, int64_t nq, int candidates, int min_count, int topk,
+                          int32_t *d_idx, int32_t *d_eq, void *stream) {
+    int rc = check_forest("dsk_forest_query_topk", d_sig, d_order, n, num_perm, weighted, l, k, d_qsig, nq);
+    if (!rc) rc = check_forest_topk("dsk_forest_query_topk", num_perm, candidates, min_count, topk, nq, d_idx, d_eq);
+    if (rc) return rc;
+    DevInfo *dev;
+    rc = current_dev(&dev);
+    if (rc) return rc;
+    DSK_CUDA(launch_forest(FOREST_QUERY_TOPK, weighted ? 2 : 1, d_sig, d_order, n, weighted ? 2 * num_perm : num_perm, l, k,
+                           d_qsig, nq, candidates, d_idx, d_eq, topk, min_count, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_forest_neighbors(const uint32_t *d_sig, const int32_t *d_order, int64_t n, int num_perm, int weighted, int l, int k,
+                         int candidates, int min_count, int topk, int32_t *d_idx, int32_t *d_eq, void *stream) {
+    int rc = check_forest("dsk_forest_neighbors", d_sig, d_order, n, num_perm, weighted, l, k, d_sig, n);
+    if (!rc) rc = check_forest_topk("dsk_forest_neighbors", num_perm, candidates, min_count, topk, n, d_idx, d_eq);
+    if (rc) return rc;
+    DevInfo *dev;
+    rc = current_dev(&dev);
+    if (rc) return rc;
+    DSK_CUDA(launch_forest(FOREST_SELF_TOPK, weighted ? 2 : 1, d_sig, d_order, n, weighted ? 2 * num_perm : num_perm, l, k,
+                           nullptr, 0, candidates, d_idx, d_eq, topk, min_count, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
 // ---- host-buffer pipeline --------------------------------------------------------------------
 extern "C++" {
 namespace {

@@ -228,6 +228,13 @@ cudaError_t launch_bbit_unpack(const uint64_t *blocks, int64_t n, int k, int slo
 cudaError_t launch_forest_query(const uint32_t *sig, const int32_t *order, int64_t n, int K, int l, int k,
                                 const uint32_t *qsig, int64_t nq, int topk, int32_t *out, int sm_count,
                                 cudaStream_t s);
+// the forest walk's modes (forest_query_kernel): the first `cap` distinct documents as a set, or ranked by eq into lists of
+// `topk` for queries (QUERY_TOPK) or for every indexed row without itself (SELF_TOPK: qsig and nq are ignored).
+// sw: words per sample (1: MinHash rows, 2: weighted MinHash rows of K = 2 * sample_size words; l and k count samples).
+enum { FOREST_SET = 0, FOREST_QUERY_TOPK = 1, FOREST_SELF_TOPK = 2 };
+cudaError_t launch_forest(int mode, int sw, const uint32_t *sig, const int32_t *order, int64_t n, int K, int l, int k,
+                          const uint32_t *qsig, int64_t nq, int cap, int32_t *idx, int32_t *eq, int topk, int min_count,
+                          int sm_count, cudaStream_t s);
 
 // ---- PTX helpers -----------------------------------------------------------------
 #ifndef DSK_EMU

@@ -228,7 +228,7 @@ cudaError_t launch_exclusive_scan(const int64_t *in, int64_t n, int64_t *out, in
 // distinct keys + per-key insertion-ordered buckets of the reference flatten to exactly this sequence.
 // warp <-> query.  For each prefix length r = k..1: lanes binary-search the l trees in parallel (tuple compare
 // on the signatures themselves), then the matches are emitted tree by tree, in sequence order, into the
-// query's result list (first `topk` DISTINCT documents), stopping exactly where the reference returns.
+// query's result list (first `cap` DISTINCT documents), stopping exactly where the reference returns.
 namespace dsk {
 
 __device__ __forceinline__ int lex_cmp(const uint32_t *a, const uint32_t *b, int r) {
@@ -239,13 +239,47 @@ __device__ __forceinline__ int lex_cmp(const uint32_t *a, const uint32_t *b, int
     return 0;
 }
 
+// The warp-held top-k list of the ranked queries (lsh_pairs_kernel's TOPK modes, forest_query_kernel's): lane j holds
+// entry j as (best_d, best_eq), -1 / -1 while empty, in the order larger eq, then smaller document number.  Every lane
+// calls it with the same candidate c and its count e.  If e >= min_count, c goes in at position popc(ballot(entry j is
+// better)): the lanes above it shift up by one shuffle and the lane at it takes c; a candidate that entry topk - 1 beats
+// changes nothing.
+__device__ __forceinline__ void topk_insert(int32_t &best_d, int32_t &best_eq, int32_t c, int e, int lane, int topk,
+                                            int min_count) {
+    const bool better = lane < topk && (best_eq > e || (best_eq == e && best_d < c));
+    const int at = __popc(__ballot_sync(0xFFFFFFFFu, better));   // entries before c
+    if (e >= min_count && at < topk) {
+        const int32_t ue = __shfl_up_sync(0xFFFFFFFFu, best_eq, 1);
+        const int32_t ud = __shfl_up_sync(0xFFFFFFFFu, best_d, 1);
+        if (lane == at) { best_eq = e; best_d = c; }
+        else if (lane > at) { best_eq = ue; best_d = ud; }
+    }
+}
+
+// MODE (FOREST_*, dsk_common.cuh):
+//   SET         out_idx[q * cap ...] = the collected list, -1 pads (MinHashLSHForest.query(m, cap)); out_eq, topk and
+//               min_count are unused
+//   QUERY_TOPK  phase 1 collects the same list of `cap` (= candidates) documents; phase 2 counts each one's eq against
+//               the query row over all K words, one document after the other across the warp, and keeps those with
+//               eq >= min_count in the warp-held list of topk_insert; lanes < topk store out_idx / out_eq [q * topk + lane]
+//   SELF_TOPK   QUERY_TOPK for index row q (the launcher passes qsig = sig, nq = n) with document q skipped while
+//               collecting -- by number, so an exact copy of q stays a candidate, and q never counts against cap
+// The filter only removes documents from the collected list: which documents are collected does not depend on it.
+// SW = words per sample.  SW = 1: MinHash rows, k and r count words.  SW = 2: weighted MinHash rows, sample s = words
+// 2s (k, uint32) and 2s + 1 (t, int32 two's complement); K = 2 * sample_size words, and tree t's samples are words
+// [2tk, 2(t+1)k).  Compared as unsigned words, these rows sort like the reference's big-endian int64 (k, t) keys (a
+// negative t sorts after every non-negative one in both), so the binary search and the emission compare 2r words for
+// a prefix of r samples -- never an odd number of words.  eq counts the samples whose two words are both equal, each
+// read with one 8-byte load (rows of 2 * sample_size words stay 8-byte aligned).
+template <int MODE, int SW>
 __global__ void __launch_bounds__(128) forest_query_kernel(const uint32_t *__restrict__ sig,
                                                            const int32_t *__restrict__ order, int64_t n, int K, int l,
                                                            int k, const uint32_t *__restrict__ qsig, int64_t nq,
-                                                           int topk, int32_t *__restrict__ out) {
-    DSK_DYNAMIC_SMEM_T(int32_t, s_res, 4);  // [warps][topk]
+                                                           int cap, int32_t *__restrict__ out_idx,
+                                                           int32_t *__restrict__ out_eq, int topk, int min_count) {
+    DSK_DYNAMIC_SMEM_T(int32_t, s_res, 4);  // [warps][cap]
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int32_t *res = s_res + warp * topk;
+    int32_t *res = s_res + warp * cap;
     const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
     for (int64_t q = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp; q < nq; q += warps) {
         const uint32_t *qrow = qsig + q * K;
@@ -256,12 +290,12 @@ __global__ void __launch_bounds__(128) forest_query_kernel(const uint32_t *__res
                 const int tree = t0 + lane;
                 int64_t lo = 0;
                 if (tree < l) {  // lower bound of the r-prefix in this lane's tree
-                    const uint32_t *qt = qrow + tree * k;
+                    const uint32_t *qt = qrow + tree * SW * k;
                     const int32_t *ord = order + (int64_t)tree * n;
                     int64_t hi = n;
                     while (lo < hi) {
                         const int64_t mid = lo + ((hi - lo) >> 1);
-                        if (lex_cmp(sig + (int64_t)ord[mid] * K + tree * k, qt, r) < 0) lo = mid + 1;
+                        if (lex_cmp(sig + (int64_t)ord[mid] * K + tree * SW * k, qt, SW * r) < 0) lo = mid + 1;
                         else hi = mid;
                     }
                 }
@@ -270,40 +304,84 @@ __global__ void __launch_bounds__(128) forest_query_kernel(const uint32_t *__res
                     int64_t pos = __shfl_sync(0xFFFFFFFFu, lo, j);
                     if (lane == 0) {
                         const int tj = t0 + j;
-                        const uint32_t *qt = qrow + tj * k;
+                        const uint32_t *qt = qrow + tj * SW * k;
                         const int32_t *ord = order + (int64_t)tj * n;
                         while (pos < n) {
                             const int32_t d = ord[pos];
-                            if (lex_cmp(sig + (int64_t)d * K + tj * k, qt, r) != 0) break;
-                            bool seen = false;
+                            if (lex_cmp(sig + (int64_t)d * K + tj * SW * k, qt, SW * r) != 0) break;
+                            bool seen = MODE == FOREST_SELF_TOPK && d == q;
                             for (int e = 0; e < cnt; ++e) seen = seen || (res[e] == d);
                             if (!seen) {
                                 res[cnt++] = d;
-                                if (cnt >= topk) break;
+                                if (cnt >= cap) break;
                             }
                             ++pos;
                         }
                     }
                     cnt = __shfl_sync(0xFFFFFFFFu, cnt, 0);
-                    done = cnt >= topk;
+                    done = cnt >= cap;
                 }
             }
         }
         __syncwarp();
-        for (int e = lane; e < topk; e += 32) out[q * topk + e] = e < cnt ? res[e] : -1;
+        if constexpr (MODE == FOREST_SET) {
+            for (int e = lane; e < cap; e += 32) out_idx[q * cap + e] = e < cnt ? res[e] : -1;
+        } else {
+            int32_t best_d = -1, best_eq = -1;   // entry `lane` of the ranked list
+            for (int e = 0; e < cnt; ++e) {
+                const int32_t c = res[e];
+                const uint32_t *crow = sig + (int64_t)c * K;
+                int m = 0;
+                if constexpr (SW == 1) {
+                    for (int w = lane; w < K; w += 32) m += crow[w] == qrow[w];
+                } else {
+                    // a sample's two words as one 64-bit value: equal iff k and t are both equal
+                    const uint64_t *c2 = reinterpret_cast<const uint64_t *>(crow);
+                    const uint64_t *q2 = reinterpret_cast<const uint64_t *>(qrow);
+                    for (int w = lane; w < (K >> 1); w += 32) m += c2[w] == q2[w];
+                }
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) m += __shfl_xor_sync(0xFFFFFFFFu, m, o);
+                topk_insert(best_d, best_eq, c, m, lane, topk, min_count);
+            }
+            if (lane < topk) { out_idx[q * topk + lane] = best_d; out_eq[q * topk + lane] = best_eq; }
+        }
         __syncwarp();
     }
+}
+
+template <int MODE, int SW>
+static cudaError_t forest_launch_t(const uint32_t *sig, const int32_t *order, int64_t n, int K, int l, int k,
+                                   const uint32_t *qsig, int64_t nq, int cap, int32_t *idx, int32_t *eq, int topk,
+                                   int min_count, int sm_count, cudaStream_t s) {
+    if (nq <= 0) return cudaSuccess;
+    int64_t grid = (nq + 3) / 4;
+    if (grid > (int64_t)sm_count * 8) grid = (int64_t)sm_count * 8;
+    const size_t smem = (size_t)4 * cap * sizeof(int32_t);
+    DSK_LAUNCH((forest_query_kernel<MODE, SW>), (unsigned)grid, 128, smem, s, sig, order, n, K, l, k, qsig, nq, cap, idx,
+               eq, topk, min_count);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_forest(int mode, int sw, const uint32_t *sig, const int32_t *order, int64_t n, int K, int l, int k,
+                          const uint32_t *qsig, int64_t nq, int cap, int32_t *idx, int32_t *eq, int topk, int min_count,
+                          int sm_count, cudaStream_t s) {
+    if (mode == FOREST_SELF_TOPK) { qsig = sig; nq = n; }
+#define DSK_FOREST_CASE(M)                                                                                                  \
+    if (mode == M)                                                                                                          \
+        return sw == 2 ? forest_launch_t<M, 2>(sig, order, n, K, l, k, qsig, nq, cap, idx, eq, topk, min_count, sm_count, s) \
+                       : forest_launch_t<M, 1>(sig, order, n, K, l, k, qsig, nq, cap, idx, eq, topk, min_count, sm_count, s);
+    DSK_FOREST_CASE(FOREST_SET)
+    DSK_FOREST_CASE(FOREST_QUERY_TOPK)
+    DSK_FOREST_CASE(FOREST_SELF_TOPK)
+#undef DSK_FOREST_CASE
+    return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_forest_query(const uint32_t *sig, const int32_t *order, int64_t n, int K, int l, int k,
                                 const uint32_t *qsig, int64_t nq, int topk, int32_t *out, int sm_count,
                                 cudaStream_t s) {
-    if (nq <= 0) return cudaSuccess;
-    int64_t grid = (nq + 3) / 4;
-    if (grid > (int64_t)sm_count * 8) grid = (int64_t)sm_count * 8;
-    const size_t smem = (size_t)4 * topk * sizeof(int32_t);
-    DSK_LAUNCH(forest_query_kernel, (unsigned)grid, 128, smem, s, sig, order, n, K, l, k, qsig, nq, topk, out);
-    return cudaGetLastError();
+    return launch_forest(FOREST_SET, 1, sig, order, n, K, l, k, qsig, nq, topk, out, nullptr, 0, 0, sm_count, s);
 }
 
 }  // namespace dsk
@@ -468,14 +546,7 @@ __global__ void __launch_bounds__(256) lsh_pairs_kernel(const LshDev ix, int64_t
                         if (lane == src) eq = e;
                         if constexpr (TOPK) {   // e and c are the same in every lane: the insert is warp-uniform
                             const int32_t c = __shfl_sync(0xFFFFFFFFu, cand, src);
-                            const bool better = lane < topk && (best_eq > e || (best_eq == e && best_d < c));
-                            const int at = __popc(__ballot_sync(0xFFFFFFFFu, better));   // entries before c
-                            if (e >= min_count && at < topk) {
-                                const int32_t ue = __shfl_up_sync(0xFFFFFFFFu, best_eq, 1);
-                                const int32_t ud = __shfl_up_sync(0xFFFFFFFFu, best_d, 1);
-                                if (lane == at) { best_eq = e; best_d = c; }
-                                else if (lane > at) { best_eq = ue; best_d = ud; }
-                            }
+                            topk_insert(best_d, best_eq, c, e, lane, topk, min_count);
                         }
                     }
                 }

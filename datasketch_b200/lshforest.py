@@ -145,16 +145,27 @@ class GpuLSHForest:
 
     ``add`` appends signatures (documents are numbered in insertion order; ``keys`` optionally maps
     numbers to user keys), ``index`` sorts every tree, ``query`` returns for each query row the same
-    document set ``MinHashLSHForest.query`` returns for the same insertion order.
+    document set ``MinHashLSHForest.query`` returns for the same insertion order.  ``query_topk`` and
+    ``neighbors`` rank the documents a walk collects by Jaccard similarity on the device.
+
+    ``weighted=True`` indexes weighted MinHash signatures, as ``MinHashLSHForest(num_perm=ss)`` does with
+    ``WeightedMinHash`` objects: ``num_perm`` is the sample size ss, ``l`` and the prefix length ``k`` count samples,
+    and every method that takes signatures takes ``[N, ss, 2]`` integer ``(k, t)`` rows (a numpy array, a CUDA tensor
+    as ``WeightedMinHashGenerator.minhash_batch(..., to_host=False)`` returns it, or a list of ``WeightedMinHash``) with
+    ``0 <= k < 2^32`` and ``-2^31 <= t < 2^31``.  The rows are held packed as ``GpuLSH(weighted=True)`` holds them
+    (sample j = word 2j = k, word 2j + 1 = t); compared as unsigned words they sort like the reference's keys, so the
+    query sets are the reference's.
     """
 
-    def __init__(self, num_perm: int = 128, l: int = 8, device: int = 0):
+    def __init__(self, num_perm: int = 128, l: int = 8, device: int = 0, weighted: bool = False):
         if l <= 0 or num_perm <= 0:
             raise ValueError("num_perm and l must be positive")
         if l > num_perm:
             raise ValueError("l cannot be greater than num_perm")
         nv.require_device(device)
         self.l, self.k, self.h = l, int(num_perm / l), num_perm
+        self.weighted = bool(weighted)
+        self.sw = 2 if self.weighted else 1          # words per sample
         self.device = device
         self._blocks: List = []
         self._sig = None
@@ -164,16 +175,21 @@ class GpuLSHForest:
     def __len__(self) -> int:
         return sum(int(b.shape[0]) for b in self._blocks)
 
-    def add(self, sig, keys: Optional[Sequence[Hashable]] = None) -> None:
+    def _dev_sig(self, sig):
         import torch
-        from .lsh import _signature_matrix
+        from .lsh import _pack_weighted, _signature_matrix
+        if self.weighted:
+            return _pack_weighted(sig, self.h, torch.device("cuda", self.device))
         if isinstance(sig, np.ndarray):
             sig = torch.from_numpy(_signature_matrix(sig).view(np.int32)).cuda(self.device)
         if sig.dim() != 2 or sig.shape[1] < self.k * self.l or sig.shape[1] != self.h:
             raise ValueError("The num_perm of MinHash out of range")
         if sig.element_size() != 4:
             raise TypeError("GpuLSHForest takes the 32-bit signature matrix")
-        self._blocks.append(sig.contiguous())
+        return sig.contiguous()
+
+    def add(self, sig, keys: Optional[Sequence[Hashable]] = None) -> None:
+        self._blocks.append(self._dev_sig(sig))
         if keys is not None:
             self.keys.extend(keys)
 
@@ -182,17 +198,20 @@ class GpuLSHForest:
 
     def index(self) -> None:
         """Sort every tree by (k-tuple, document number): stable LSD passes over pairs of columns
-        (``torch.sort`` is used as the sort primitive; the query walk is the hand-written kernel)."""
+        (``torch.sort`` is used as the sort primitive; the query walk is the hand-written kernel).  On a weighted
+        forest a tree spans 2k words and each pair of columns is one ``(k, t)`` sample."""
         import torch
-        self._sig = torch.cat(self._blocks, 0) if self._blocks else torch.zeros((0, self.h), dtype=torch.int32,
+        width = self.sw * self.h
+        self._sig = torch.cat(self._blocks, 0) if self._blocks else torch.zeros((0, width), dtype=torch.int32,
                                                                              device=torch.device("cuda", self.device))
         self._blocks = [self._sig] if len(self._sig) else []
         n = self._sig.shape[0]
         u = self._sig.to(torch.int64) & 0xFFFFFFFF
+        kw = self.sw * self.k                        # words per tree
         orders = []
         for t in range(self.l):
             order = torch.arange(n, device=self._sig.device)
-            cols = list(range(t * self.k, (t + 1) * self.k))
+            cols = list(range(t * kw, (t + 1) * kw))
             while cols:
                 hi_lo = cols[-2:]
                 cols = cols[:-2]
@@ -204,30 +223,108 @@ class GpuLSHForest:
             orders.append(order.to(torch.int32))
         self._order = torch.stack(orders) if orders else None
 
+    def _indexed(self):
+        if self._order is None:
+            raise ValueError("index() has not been called")
+        n = self._sig.shape[0]
+        return (self._sig.data_ptr() if n else None), (self._order.data_ptr() if n else None), n
+
     def query(self, sig, k: int, to_host: bool = True):
         """[Q, K] query signatures -> int32 [Q, k] document numbers (-1 pads), per row the set the
         reference's ``query(minhash, k)`` returns."""
         import torch
-        from .lsh import _signature_matrix
         if k <= 0:
             raise ValueError("k must be positive")
-        if self._order is None:
-            raise ValueError("index() has not been called")
-        if isinstance(sig, np.ndarray):
-            sig = torch.from_numpy(_signature_matrix(sig).view(np.int32)).cuda(self.device)
-        if sig.dim() != 2 or sig.shape[1] != self.h:
-            raise ValueError("The num_perm of MinHash out of range")
-        if sig.element_size() != 4:
-            raise TypeError("GpuLSHForest takes the 32-bit signature matrix")
-        sig = sig.contiguous()
-        nq, n = sig.shape[0], self._sig.shape[0]
+        d_sig, d_order, n = self._indexed()
+        sig = self._dev_sig(sig)
+        nq = sig.shape[0]
         out = torch.empty((nq, k), dtype=torch.int32, device=sig.device)
         with torch.cuda.device(self.device):
-            nv.check(nv.load().dsk_forest_query(self._sig.data_ptr() if n else None, self._order.data_ptr() if n else None,
-                                                n, self.h, self.l, self.k, sig.data_ptr(), nq, k, out.data_ptr(),
-                                                torch.cuda.current_stream().cuda_stream))
+            st = torch.cuda.current_stream().cuda_stream
+            if self.weighted:
+                nv.check(nv.load().dsk_forest_query_weighted(d_sig, d_order, n, self.h, self.l, self.k, sig.data_ptr(), nq,
+                                                             k, out.data_ptr(), st))
+            else:
+                nv.check(nv.load().dsk_forest_query(d_sig, d_order, n, self.h, self.l, self.k, sig.data_ptr(), nq, k,
+                                                    out.data_ptr(), st))
         return out.cpu().numpy() if to_host else out
 
     def query_keys(self, sig, k: int) -> List[list]:
         res = self.query(sig, k)
         return [[(self.keys[i] if self.keys else int(i)) for i in row if i >= 0] for row in res]
+
+    # -- ranked answers: the reference docstring's post-processing, on the device -------------------------------------
+    @staticmethod
+    def _check_candidates(candidates, k: int) -> int:
+        if candidates is None:
+            candidates = 2 * k
+        if isinstance(candidates, bool) or not isinstance(candidates, (int, np.integer)) or not k <= candidates <= 1024:
+            raise ValueError("candidates must be an integer in [k, 1024], got %r" % (candidates,))
+        return int(candidates)
+
+    def query_topk(self, sig, k: int, candidates: Optional[int] = None, min_jaccard: Optional[float] = None,
+                   to_host: bool = True):
+        """Each query's k most similar documents among its forest candidates: ``(idx int32[Q, k], eq int32[Q, k])``.
+
+        The reference's ``query`` docstring suggests asking for a multiple of k and keeping the k best by Jaccard
+        similarity; this does that on the device.  For query m, row q is::
+
+            cand = forest.query(m, candidates)          # the set query(sig, candidates) returns
+            sorted([d for d in cand if m.jaccard(doc[d]) >= t], key=lambda d: (-m.jaccard(doc[d]), d))[:k]
+
+        with -1 / -1 behind the list.  ``eq`` counts the equal positions over all ``num_perm`` (on a weighted forest:
+        the samples whose whole ``(k, t)`` pairs agree), so ``eq / num_perm`` is ``MinHash.jaccard`` /
+        ``WeightedMinHash.jaccard``; columns past ``l * k``, which the walk never reads, count too.  ``k`` is in
+        ``[1, 32]``, ``candidates`` (default ``2 * k``) in ``[k, 1024]``.  ``min_jaccard`` only removes documents from
+        the collected set; it never changes which are collected.  One launch, no host synchronisation, and an output
+        of ``Q * k`` entries."""
+        import torch
+        from .lsh import _check_topk, _jaccard_min_count
+        k = _check_topk(k)
+        candidates = self._check_candidates(candidates, k)
+        mc = _jaccard_min_count(min_jaccard, self.h)
+        d_sig, d_order, n = self._indexed()
+        sig = self._dev_sig(sig)
+        nq = sig.shape[0]
+        with torch.cuda.device(self.device):
+            idx = torch.empty((max(nq, 1), k), dtype=torch.int32, device=sig.device)
+            eq = torch.empty((max(nq, 1), k), dtype=torch.int32, device=sig.device)
+            nv.check(nv.load().dsk_forest_query_topk(d_sig, d_order, n, self.h, int(self.weighted), self.l, self.k,
+                                                     sig.data_ptr() if nq else None, nq, candidates, mc, k,
+                                                     idx.data_ptr(), eq.data_ptr(), torch.cuda.current_stream().cuda_stream))
+            idx, eq = idx[:nq], eq[:nq]
+        if to_host:
+            return idx.cpu().numpy(), eq.cpu().numpy()
+        return idx, eq
+
+    def neighbors(self, k: int, candidates: Optional[int] = None, min_jaccard: Optional[float] = None,
+                  to_host: bool = True):
+        """The k nearest neighbours of every indexed document, with no LSH threshold: ``(idx int32[n, k], eq int32[n, k])``.
+
+        Row i ranks, as ``query_topk`` does, the first ``candidates`` distinct documents other than i that the forest
+        walk of document i's own row meets -- in reference terms::
+
+            res = set()
+            for r in range(forest.k, 0, -1):
+                for d in forest._query(doc[i], r, forest.l):
+                    if d != i: res.add(d)
+                    if len(res) >= candidates: stop both loops
+
+        The test is by document number, so an exact copy of i stays a neighbour.  One launch, no host synchronisation."""
+        import torch
+        from .lsh import _check_topk, _jaccard_min_count
+        k = _check_topk(k)
+        candidates = self._check_candidates(candidates, k)
+        mc = _jaccard_min_count(min_jaccard, self.h)
+        d_sig, d_order, n = self._indexed()
+        with torch.cuda.device(self.device):
+            dev = torch.device("cuda", self.device)
+            idx = torch.empty((max(n, 1), k), dtype=torch.int32, device=dev)
+            eq = torch.empty((max(n, 1), k), dtype=torch.int32, device=dev)
+            nv.check(nv.load().dsk_forest_neighbors(d_sig, d_order, n, self.h, int(self.weighted), self.l, self.k,
+                                                    candidates, mc, k, idx.data_ptr(), eq.data_ptr(),
+                                                    torch.cuda.current_stream().cuda_stream))
+            idx, eq = idx[:n], eq[:n]
+        if to_host:
+            return idx.cpu().numpy(), eq.cpu().numpy()
+        return idx, eq

@@ -469,6 +469,29 @@ DSK_API int dsk_jaccard_topk_ws(const uint32_t *d_q, int64_t nq, const uint32_t 
 DSK_API int dsk_forest_query(const uint32_t *d_sig, const int32_t *d_order, int64_t n, int num_perm, int l, int k,
                              const uint32_t *d_qsig, int64_t nq, int topk, int32_t *d_out, void *stream);
 
+/* Weighted MinHash rows (MinHashLSHForest over WeightedMinHash): d_sig / d_qsig are [n, 2 * sample_size] u32, sample j
+ * packed as word 2j = k_j (uint32) and word 2j + 1 = t_j (int32, two's complement), 8-byte aligned; l, k and
+ * sample_size count samples.  Compared as unsigned words, such rows sort like the reference's big-endian int64 (k, t)
+ * keys, so d_order is built exactly as above over the tree's 2k words, and the walk compares 2r words for a prefix of
+ * r samples.  Otherwise as dsk_forest_query. */
+DSK_API int dsk_forest_query_weighted(const uint32_t *d_sig, const int32_t *d_order, int64_t n, int sample_size, int l,
+                                      int k, const uint32_t *d_qsig, int64_t nq, int topk, int32_t *d_out, void *stream);
+/* Ranked forest queries.  weighted = 0: rows of num_perm words; weighted = 1: rows as dsk_forest_query_weighted's, with
+ * num_perm the sample size.  For each query the walk collects the first `candidates` (topk <= candidates <= 1024)
+ * distinct documents dsk_forest_query(..., candidates) would return; then eq[d] = the number of positions (samples,
+ * whole (k, t) pairs) among all num_perm where the rows agree -- eq / num_perm is MinHash.jaccard / WeightedMinHash.jaccard
+ * -- and the collected documents with eq >= min_count (0 <= min_count <= num_perm) are ranked by larger eq, then smaller
+ * number.  d_idx / d_eq [nq, topk] (1 <= topk <= 32) hold the first topk of them, -1 / -1 behind.  The filter never
+ * changes which documents are collected.  One launch, no workspace. */
+DSK_API int dsk_forest_query_topk(const uint32_t *d_sig, const int32_t *d_order, int64_t n, int num_perm, int weighted,
+                                  int l, int k, const uint32_t *d_qsig, int64_t nq, int candidates, int min_count, int topk,
+                                  int32_t *d_idx, int32_t *d_eq, void *stream);
+/* The same ranking for every indexed row i ([n, topk] outputs): the walk of row i collects the first `candidates`
+ * distinct documents other than i (by number: an exact copy of i is collected; i never counts against candidates). */
+DSK_API int dsk_forest_neighbors(const uint32_t *d_sig, const int32_t *d_order, int64_t n, int num_perm, int weighted,
+                                 int l, int k, int candidates, int min_count, int topk, int32_t *d_idx, int32_t *d_eq,
+                                 void *stream);
+
 /* ---- b-bit MinHash blocks ("next" row, SURVEY.md 8f) -----------------------------------------
  * bBitMinHash keeps the b lowest bits of each value (datasketch/b_bit_minhash.py:38) and packs
  * them into 64-bit blocks, value j of a block at bit (n-1-j)*slot with slot = 1,2,4,8,16,32 >= b
