@@ -78,6 +78,15 @@ SIGNATURES = {
     "dsk_lsh_ensemble_index": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "dsk_lsh_ensemble_query_count": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "dsk_lsh_ensemble_query_fill": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dsk_lsh_ensemble_containment_count": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, ctypes.c_double,
+                                                   c_void_p, c_void_p]),
+    "dsk_lsh_ensemble_containment_fill": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, ctypes.c_double,
+                                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dsk_lsh_ensemble_containment_topk": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, ctypes.c_double,
+                                                  c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dsk_lsh_ensemble_self_containment_count": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_double, c_void_p, c_void_p]),
+    "dsk_lsh_ensemble_self_containment_fill": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_double, c_void_p, c_void_p,
+                                                       c_void_p, c_void_p, c_void_p]),
     "dsk_ensemble_partition_workspace_size": (ctypes.c_size_t, [c_int64, c_int]),
     "dsk_ensemble_partition": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p, ctypes.c_size_t, c_int, c_void_p,
                                        c_void_p, c_void_p]),

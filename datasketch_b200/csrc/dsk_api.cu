@@ -1449,6 +1449,107 @@ int dsk_lsh_ensemble_query_fill(const dsk_lsh_ensemble *e, const uint32_t *d_qsi
     return DSK_OK;
 }
 
+// check_ensemble_query, plus min_containment in [0, 1] (NaN fails both comparisons)
+static int check_ensemble_containment(const char *who, const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq,
+                                      const int32_t *d_sel, bool bufs, double min_containment) {
+    int rc = check_ensemble_query(who, e, d_qsig, nq, d_sel, bufs);
+    if (rc) return rc;
+    if (!(min_containment >= 0.0 && min_containment <= 1.0)) {
+        set_error("%s: min_containment must be in [0, 1] (got %g)", who, min_containment);
+        return DSK_ERR_INVALID;
+    }
+    return DSK_OK;
+}
+
+// the count and fill of the query and self-join flavours; qsig == nullptr is the self-join (nq = the number of sets)
+static int ensemble_containment_call(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int64_t *d_qsizes,
+                                     const int32_t *d_sel, const int64_t *d_set_sizes, double min_containment,
+                                     int64_t *d_counts, const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq,
+                                     double *d_containment, void *stream) {
+    DevGuard guard(e->device);
+    if (e->n_sets == 0) {   // nothing indexed: no candidates
+        if (d_counts) DSK_CUDA(cudaMemsetAsync(d_counts, 0, (size_t)nq * e->dev.num_part * 8, (cudaStream_t)stream));
+        return DSK_OK;
+    }
+    DevInfo *dev;
+    int rc = get_dev(e->device, &dev);
+    if (rc) return rc;
+    DSK_CUDA(ensemble_containment(e->dev, d_qsig, nq, d_qsizes, d_sel, d_set_sizes, min_containment, d_counts, d_ptr, d_idx,
+                                  d_eq, d_containment, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_lsh_ensemble_containment_count(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int64_t *d_qsizes,
+                                       const int32_t *d_sel, const int64_t *d_set_sizes, double min_containment,
+                                       int64_t *d_counts, void *stream) {
+    int rc = check_ensemble_containment("dsk_lsh_ensemble_containment_count", e, d_qsig, nq, d_sel,
+                                        d_qsizes && d_set_sizes && d_counts, min_containment);
+    if (rc || nq == 0) return rc;
+    return ensemble_containment_call(e, d_qsig, nq, d_qsizes, d_sel, d_set_sizes, min_containment, d_counts, nullptr, nullptr,
+                                     nullptr, nullptr, stream);
+}
+
+int dsk_lsh_ensemble_containment_fill(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int64_t *d_qsizes,
+                                      const int32_t *d_sel, const int64_t *d_set_sizes, double min_containment,
+                                      const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq, double *d_containment,
+                                      void *stream) {
+    int rc = check_ensemble_containment("dsk_lsh_ensemble_containment_fill", e, d_qsig, nq, d_sel,
+                                        d_qsizes && d_set_sizes && d_ptr && d_idx && d_eq && d_containment, min_containment);
+    if (rc || nq == 0) return rc;
+    return ensemble_containment_call(e, d_qsig, nq, d_qsizes, d_sel, d_set_sizes, min_containment, nullptr, d_ptr, d_idx,
+                                     d_eq, d_containment, stream);
+}
+
+int dsk_lsh_ensemble_containment_topk(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int64_t *d_qsizes,
+                                      const int32_t *d_sel, const int64_t *d_set_sizes, double min_containment, int k,
+                                      int32_t *d_idx, int32_t *d_eq, double *d_containment, void *stream) {
+    const char *who = "dsk_lsh_ensemble_containment_topk";
+    int rc = check_ensemble_containment(who, e, d_qsig, nq, d_sel, d_qsizes && d_set_sizes && d_idx && d_eq && d_containment,
+                                        min_containment);
+    if (rc) return rc;
+    if (k < 1 || k > 32) {
+        set_error("%s: k must be in [1, 32] (got %d)", who, k);
+        return DSK_ERR_INVALID;
+    }
+    if (nq == 0) return DSK_OK;
+    DevInfo *dev;
+    rc = get_dev(e->device, &dev);
+    if (rc) return rc;
+    DevGuard guard(e->device);
+    DSK_CUDA(ensemble_containment_topk(e->dev, d_qsig, nq, d_qsizes, d_sel, d_set_sizes, min_containment, k, d_idx, d_eq,
+                                       d_containment, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_lsh_ensemble_self_containment_count(const dsk_lsh_ensemble *e, const int32_t *d_sel, const int64_t *d_set_sizes,
+                                            double min_containment, int64_t *d_counts, void *stream) {
+    const char *who = "dsk_lsh_ensemble_self_containment_count";
+    const int64_t n = e ? e->n_sets : 0;
+    int rc = check_ensemble_containment(who, e, nullptr, 0, d_sel, true, min_containment);
+    if (rc || n == 0) return rc;
+    if (!d_sel || !d_set_sizes || !d_counts) {
+        set_error("%s: null buffer", who);
+        return DSK_ERR_INVALID;
+    }
+    return ensemble_containment_call(e, nullptr, n, nullptr, d_sel, d_set_sizes, min_containment, d_counts, nullptr, nullptr,
+                                     nullptr, nullptr, stream);
+}
+
+int dsk_lsh_ensemble_self_containment_fill(const dsk_lsh_ensemble *e, const int32_t *d_sel, const int64_t *d_set_sizes,
+                                           double min_containment, const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq,
+                                           double *d_containment, void *stream) {
+    const char *who = "dsk_lsh_ensemble_self_containment_fill";
+    const int64_t n = e ? e->n_sets : 0;
+    int rc = check_ensemble_containment(who, e, nullptr, 0, d_sel, true, min_containment);
+    if (rc || n == 0) return rc;
+    if (!d_sel || !d_set_sizes || !d_ptr || !d_idx || !d_eq || !d_containment) {
+        set_error("%s: null buffer", who);
+        return DSK_ERR_INVALID;
+    }
+    return ensemble_containment_call(e, nullptr, n, nullptr, d_sel, d_set_sizes, min_containment, nullptr, d_ptr, d_idx, d_eq,
+                                     d_containment, stream);
+}
+
 // ---- MinHashLSHEnsemble's size partitioner -------------------------------------------------------------------------------
 // acc += a * b rounded up to 256 bytes; false if it does not fit in size_t
 static bool ws_add(size_t &acc, uint64_t a, uint64_t b) {

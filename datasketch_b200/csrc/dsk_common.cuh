@@ -196,6 +196,14 @@ cudaError_t ensemble_index(const EnsembleDev &en, const uint32_t *rows, const in
                            cudaStream_t s);
 cudaError_t ensemble_query(const EnsembleDev &en, const uint32_t *qsig, int64_t nq, const int32_t *sel, int64_t *counts,
                            const int64_t *ptr, int32_t *idx, int32_t *eq, int sm_count, cudaStream_t s);
+// containment estimates of the query candidates (qsig != nullptr) or of the self-join (qsig == nullptr, nq = n): counts, or
+// the fill of idx / eq / c at ptr; only candidates with c >= min_c.  set_sizes: int64[n] in the index call's row order.
+cudaError_t ensemble_containment(const EnsembleDev &en, const uint32_t *qsig, int64_t nq, const int64_t *qsizes,
+                                 const int32_t *sel, const int64_t *set_sizes, double min_c, int64_t *counts,
+                                 const int64_t *ptr, int32_t *idx, int32_t *eq, double *c, int sm_count, cudaStream_t s);
+cudaError_t ensemble_containment_topk(const EnsembleDev &en, const uint32_t *qsig, int64_t nq, const int64_t *qsizes,
+                                      const int32_t *sel, const int64_t *set_sizes, double min_c, int topk, int32_t *idx,
+                                      int32_t *eq, double *c, int sm_count, cudaStream_t s);
 // the size partitioner over n distinct sizes (device copies of sizes / counts): the cost triangle, and with tab != nullptr
 // (2 <= num_part < n; num_part - 1 rows of n doubles) the dynamic programme and the upper index of each partition into
 // upper[num_part].  g_terms: partition_term_rows(n) rows of n doubles (none while a column's terms fit shared memory).

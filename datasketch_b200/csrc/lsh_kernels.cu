@@ -1362,6 +1362,244 @@ cudaError_t ensemble_query(const EnsembleDev &en, const uint32_t *qsig, int64_t 
     return cudaGetLastError();
 }
 
+// ---- containment estimates of the ensemble's candidates ---------------------------------------------------------------------
+// c = j * (s_q + s_x) / (s_q * (1 + j)), j = eq / K: the inverse of the map t -> t / (1 + x/q - t) that turns a containment
+// into the Jaccard value the (b, r) table was chosen for (lshensemble.py's _false_positive_probability), so c estimates
+// |Q & X| / |Q|.  Evaluated as the Python expression over ints and floats is: every operation rounded on its own (no FMA
+// contraction, no reciprocal), the int sum s_q + s_x exact (both sizes below 2^62) and converted once.
+__device__ __forceinline__ double containment_est(int eq, int k, int64_t sq, int64_t sx) {
+    const double j = __ddiv_rn((double)eq, (double)k);
+    return __ddiv_rn(__dmul_rn(j, __ll2double_rn(sq + sx)), __dmul_rn(__ll2double_rn(sq), __dadd_rn(1.0, j)));
+}
+
+// ensemble_query_kernel's walk of one (query, partition) item with table row s, the query row in row[0..k): lane <-> band < b
+// (further rounds beyond 32), the chain walk to each lane's next candidate (inside [lo, hi), not set number `skip`, the tuple
+// really equal, no earlier band equal), and emit(pending, cand) for each round of candidates, warp-uniformly.
+template <class Emit>
+__device__ __forceinline__ void ensemble_walk(const EnsembleDev &en, const uint32_t *row, int part, int s, int64_t lo,
+                                              int64_t hi, int64_t skip, int lane, Emit &&emit) {
+    const int k = en.tab[0].k;
+    const int nb = en.pb[s];
+    const LshDev &ix = en.tab[en.pt[s]];
+    const uint64_t mask = (uint64_t)ix.cap_slots - 1;
+    for (int band0 = 0; band0 < nb; band0 += 32) {
+        const int band = band0 + lane;
+        const uint32_t *qt = row + band * ix.r;
+        int32_t d = -1;
+        if (band < nb) {
+            const uint64_t fp = ensemble_fp(qt, ix.r, band, part);
+            const uint64_t *tab = ix.slots + (int64_t)band * ix.cap_slots * 2;
+            uint64_t slot = lsh_mix64(fp) & mask;
+            while (true) {
+                const uint64_t kk = tab[2 * slot];
+                if (kk == fp) { d = *reinterpret_cast<const int32_t *>(tab + 2 * slot + 1); break; }
+                if (kk == kEmptyKey) break;
+                slot = (slot + 1) & mask;
+            }
+        }
+        while (true) {
+            int32_t cand = -1;
+            while (d >= 0) {
+                const int32_t cur = d;
+                d = ix.next[(int64_t)cur * ix.b + band];
+                if (cur >= lo && cur < hi && cur != skip) {
+                    const uint32_t *drow = ix.sig + (int64_t)cur * k;
+                    if (tuple_eq(drow + band * ix.r, qt, ix.r)) {
+                        bool dup = false;
+                        for (int j = 0; j < band && !dup; ++j)
+                            dup = tuple_eq(drow + j * ix.r, row + j * ix.r, ix.r);
+                        if (!dup) { cand = cur; break; }
+                    }
+                }
+            }
+            const unsigned pending = __ballot_sync(0xFFFFFFFFu, cand >= 0);
+            if (pending == 0u) break;
+            emit(pending, cand);
+        }
+    }
+}
+
+// eq of each pending lane's candidate against row[0..k), the warp comparing one candidate's row at a time (ENS_FILL_EQ's)
+__device__ __forceinline__ int ensemble_pending_eq(const uint32_t *sig, int k, const uint32_t *row, unsigned pending,
+                                                   int32_t cand, int lane) {
+    int eq = 0;
+    for (unsigned m = pending; m; m &= m - 1u) {
+        const int src = __ffs(m) - 1;
+        const uint32_t *crow = sig + (int64_t)__shfl_sync(0xFFFFFFFFu, cand, src) * k;
+        int e = 0;
+        for (int w = lane; w < k; w += 32) e += crow[w] == row[w];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) e += __shfl_xor_sync(0xFFFFFFFFu, e, o);
+        if (lane == src) eq = e;
+    }
+    return eq;
+}
+
+enum { ENSC_COUNT = 0, ENSC_FILL = 1 };
+
+// warp <-> item, as ensemble_query_kernel, keeping the candidates x with containment_est(eq, K, s_q, s_x) >= min_c; s_x =
+// set_sizes[map[x]] (the caller's row order).  SELF = false: item q * num_part + p of the nq query rows, s_q = qsizes[q].
+// SELF = true: the walk goes over set numbers t (nq = n): the query is the index's own row t, s_q = set_sizes[map[t]], set t
+// itself is skipped (by number: an identical row is still a candidate) and the item is written (and sel read) at
+// map[t] * num_part + p, so the output is in the caller's row order.
+//   ENSC_COUNT  counts[item] = number of kept candidates (eq is only counted when min_c > 0: every c is >= 0)
+//   ENSC_FILL   out_idx / out_eq / out_c [ptr[item] ...) = row, eq and c of each kept candidate, in no particular order
+template <int MODE, bool SELF>
+__global__ void __launch_bounds__(256) ensemble_containment_kernel(
+        const EnsembleDev en, const uint32_t *__restrict__ qsig, int64_t nq, const int64_t *__restrict__ qsizes,
+        const int32_t *__restrict__ sel, const int64_t *__restrict__ set_sizes, double min_c, int64_t *__restrict__ counts,
+        const int64_t *__restrict__ ptr, int32_t *__restrict__ out_idx, int32_t *__restrict__ out_eq,
+        double *__restrict__ out_c) {
+    DSK_DYNAMIC_SMEM_T(uint32_t, s_rows, 16);   // [warps][k]
+    const int lane = threadIdx.x & 31;
+    const int k = en.tab[0].k;
+    uint32_t *row = s_rows + (int64_t)(threadIdx.x >> 5) * k;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    const unsigned below = (1u << lane) - 1u;
+    const int64_t n_items = nq * en.num_part;
+    const bool need_eq = MODE == ENSC_FILL || min_c > 0.0;
+    for (int64_t item = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < n_items; item += warps) {
+        const int64_t q = item / en.num_part;
+        const int part = (int)(item - q * en.num_part);
+        const int64_t out_item = SELF ? (int64_t)en.map[q] * en.num_part + part : item;
+        const int s = sel[out_item];
+        const int64_t lo = en.part_start[part], hi = en.part_start[part + 1];
+        if (s < 0 || s >= en.n_params || lo >= hi) {   // warp-uniform
+            if (MODE == ENSC_COUNT && lane == 0) counts[out_item] = 0;
+            continue;
+        }
+        const uint32_t *qrow = SELF ? en.tab[0].sig + q * k : qsig + q * k;
+        const int64_t sq = SELF ? set_sizes[en.map[q]] : qsizes[q];
+        __syncwarp();
+        for (int w = lane; w < k; w += 32) row[w] = qrow[w];
+        __syncwarp();
+        int64_t total = 0;   // kept candidates so far (the same in every lane)
+        ensemble_walk(en, row, part, s, lo, hi, SELF ? q : -1, lane, [&](unsigned pending, int32_t cand) {
+            int eq = 0;
+            int32_t x = -1;
+            double c = 0.0;
+            if (need_eq) {
+                eq = ensemble_pending_eq(en.tab[0].sig, k, row, pending, cand, lane);
+                if (cand >= 0) {
+                    x = en.map[cand];
+                    c = containment_est(eq, k, sq, set_sizes[x]);
+                }
+            }
+            const bool keep = cand >= 0 && (!need_eq || c >= min_c);
+            const unsigned kept = __ballot_sync(0xFFFFFFFFu, keep);
+            if (MODE == ENSC_FILL && keep) {
+                const int64_t pos = ptr[out_item] + total + __popc(kept & below);
+                out_idx[pos] = x;
+                out_eq[pos] = eq;
+                out_c[pos] = c;
+            }
+            total += __popc(kept);
+        });
+        if (MODE == ENSC_COUNT && lane == 0) counts[out_item] = total;
+    }
+}
+
+// The warp-held list of ensemble_containment_topk_kernel: lane j holds entry j as (best_c, best_x, best_eq), -1.0 / -1 / -1
+// while empty, in the order larger c, then smaller row x; topk_insert's shift, keyed by (c, x).
+__device__ __forceinline__ void topk_insert_c(double &best_c, int32_t &best_x, int32_t &best_eq, double c, int32_t x, int eq,
+                                              int lane, int topk) {
+    const bool better = lane < topk && (best_c > c || (best_c == c && best_x < x));
+    const int at = __popc(__ballot_sync(0xFFFFFFFFu, better));   // entries before (c, x)
+    if (at < topk) {
+        const double uc = __shfl_up_sync(0xFFFFFFFFu, best_c, 1);
+        const int32_t ux = __shfl_up_sync(0xFFFFFFFFu, best_x, 1);
+        const int32_t ue = __shfl_up_sync(0xFFFFFFFFu, best_eq, 1);
+        if (lane == at) { best_c = c; best_x = x; best_eq = eq; }
+        else if (lane > at) { best_c = uc; best_x = ux; best_eq = ue; }
+    }
+}
+
+// warp <-> query q: the walk of each of its partitions in turn, every candidate with c >= min_c into the warp-held list (a
+// query's candidates are disjoint across partitions, and the first-band rule emits each once within one, so no merge is
+// needed); lanes < topk store out_idx / out_eq / out_c [q * topk + lane].  An index never built (map == nullptr) pads.
+__global__ void __launch_bounds__(256) ensemble_containment_topk_kernel(
+        const EnsembleDev en, const uint32_t *__restrict__ qsig, int64_t nq, const int64_t *__restrict__ qsizes,
+        const int32_t *__restrict__ sel, const int64_t *__restrict__ set_sizes, double min_c, int topk,
+        int32_t *__restrict__ out_idx, int32_t *__restrict__ out_eq, double *__restrict__ out_c) {
+    DSK_DYNAMIC_SMEM_T(uint32_t, s_rows, 16);   // [warps][k]
+    const int lane = threadIdx.x & 31;
+    const int k = en.tab[0].k;
+    uint32_t *row = s_rows + (int64_t)(threadIdx.x >> 5) * k;
+    const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+    const int n_part = en.map ? en.num_part : 0;
+    for (int64_t q = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); q < nq; q += warps) {
+        const int64_t sq = qsizes[q];
+        __syncwarp();
+        for (int w = lane; w < k; w += 32) row[w] = qsig[q * k + w];
+        __syncwarp();
+        double best_c = -1.0;
+        int32_t best_x = -1, best_eq = -1;
+        for (int part = 0; part < n_part; ++part) {
+            const int s = sel[q * en.num_part + part];
+            const int64_t lo = en.part_start[part], hi = en.part_start[part + 1];
+            if (s < 0 || s >= en.n_params || lo >= hi) continue;   // warp-uniform
+            ensemble_walk(en, row, part, s, lo, hi, -1, lane, [&](unsigned pending, int32_t cand) {
+                const int eq = ensemble_pending_eq(en.tab[0].sig, k, row, pending, cand, lane);
+                const int32_t x = cand >= 0 ? en.map[cand] : -1;
+                const double c = x >= 0 ? containment_est(eq, k, sq, set_sizes[x]) : -1.0;
+                for (unsigned m = __ballot_sync(0xFFFFFFFFu, x >= 0 && c >= min_c); m; m &= m - 1u) {
+                    const int src = __ffs(m) - 1;
+                    topk_insert_c(best_c, best_x, best_eq, __shfl_sync(0xFFFFFFFFu, c, src),
+                                  __shfl_sync(0xFFFFFFFFu, x, src), __shfl_sync(0xFFFFFFFFu, eq, src), lane, topk);
+                }
+            });
+        }
+        if (lane < topk) {
+            out_idx[q * topk + lane] = best_x;
+            out_eq[q * topk + lane] = best_eq;
+            out_c[q * topk + lane] = best_c;
+        }
+    }
+}
+
+// counts != nullptr: counts[item] for the nq * num_part items; else the fill of idx / eq / c at ptr[item].  qsig == nullptr:
+// the self-join (nq = the number of sets, the index's own rows and set_sizes as the queries' sizes).
+cudaError_t ensemble_containment(const EnsembleDev &en, const uint32_t *qsig, int64_t nq, const int64_t *qsizes,
+                                 const int32_t *sel, const int64_t *set_sizes, double min_c, int64_t *counts,
+                                 const int64_t *ptr, int32_t *idx, int32_t *eq, double *c, int sm_count, cudaStream_t s) {
+    const int64_t n_items = nq * en.num_part;
+    if (n_items <= 0) return cudaSuccess;
+    const int k = en.tab[0].k;
+    int w = 8;
+    while (w > 1 && (size_t)w * k * 4 > 48 * 1024) w >>= 1;
+    const size_t smem = (size_t)w * k * 4;
+    int64_t g = (n_items + w - 1) / w;
+    if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
+    const unsigned grid = (unsigned)g;
+    auto launch = [&](auto kernel) {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        DSK_LAUNCH(kernel, grid, 32 * w, smem, s, en, qsig, nq, qsizes, sel, set_sizes, min_c, counts, ptr, idx, eq, c);
+        return cudaGetLastError();
+    };
+    if (qsig) return counts ? launch(ensemble_containment_kernel<ENSC_COUNT, false>)
+                            : launch(ensemble_containment_kernel<ENSC_FILL, false>);
+    return counts ? launch(ensemble_containment_kernel<ENSC_COUNT, true>) : launch(ensemble_containment_kernel<ENSC_FILL, true>);
+}
+
+cudaError_t ensemble_containment_topk(const EnsembleDev &en, const uint32_t *qsig, int64_t nq, const int64_t *qsizes,
+                                      const int32_t *sel, const int64_t *set_sizes, double min_c, int topk, int32_t *idx,
+                                      int32_t *eq, double *c, int sm_count, cudaStream_t s) {
+    if (nq <= 0) return cudaSuccess;
+    const int k = en.tab[0].k;
+    int w = 8;
+    while (w > 1 && (size_t)w * k * 4 > 48 * 1024) w >>= 1;
+    const size_t smem = (size_t)w * k * 4;
+    int64_t g = (nq + w - 1) / w;
+    if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
+    cudaError_t e = cudaFuncSetAttribute(ensemble_containment_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
+    if (e != cudaSuccess) return e;
+    DSK_LAUNCH(ensemble_containment_topk_kernel, (unsigned)g, 32 * w, smem, s, en, qsig, nq, qsizes, sel, set_sizes, min_c,
+               topk, idx, eq, c);
+    return cudaGetLastError();
+}
+
 }  // namespace dsk
 
 // ---- MinHashLSHEnsemble's size partitioner (lshensemble.py:81-120 = lshensemble_partition.py:54-196) ----------------------

@@ -359,6 +359,8 @@ class GpuLSHEnsemble:
         self.keys: Optional[list] = None
         self._keyset: Optional[set] = None
         self._start = np.zeros(num_part + 1, dtype=np.int64)
+        self._set_sizes: Optional[np.ndarray] = None   # int64[N] of the index call, in its row order
+        self._d_set_sizes = None                        # their device copy, made by the first call that needs it
         from . import _native as nv
         nv.require_device(device)
         b = np.ascontiguousarray(self.params[:, 0], dtype=np.int32)
@@ -444,6 +446,7 @@ class GpuLSHEnsemble:
             nv.check(nv.load().dsk_lsh_ensemble_index(self._h, d_sig.data_ptr(), n, d_order.data_ptr(), start.ctypes.data,
                                                       torch.cuda.current_stream().cuda_stream))
         self.lowers, self.uppers, self._start = lowers, uppers, start
+        self._set_sizes, self._d_set_sizes = sizes, None
         if keys is not None:
             self.keys, self._keyset = keys, set(keys)
 
@@ -498,3 +501,127 @@ class GpuLSHEnsemble:
             ids = idx[ptr[q]:ptr[q + 1]]
             out.append([self.keys[i] for i in ids] if self.keys is not None else ids.tolist())
         return out
+
+    # -- containment estimates on the device -----------------------------------------------------------------------
+    def _containment_args(self, sig, sizes, min_containment):
+        """The query matrix, its sizes (host and device), the device copy of the indexed sizes (a placeholder before
+        ``index``: nothing reads it) and the threshold as a float.  Query sizes must be in [1, 2^62) so that s_q + s_x
+        fits in int64."""
+        import torch
+        d_q = self._dev_sig(sig)
+        sizes = self._sizes(sizes, int(d_q.shape[0]))
+        if np.any(sizes <= 0) or np.any(sizes >= 1 << 62):
+            raise ValueError("query set sizes must be in [1, 2^62)")
+        d_xs = self._device_set_sizes()
+        if d_xs is None:
+            d_xs = torch.zeros((1,), dtype=torch.int64, device=d_q.device)
+        return d_q, sizes, torch.from_numpy(sizes).to(d_q.device), d_xs, _min_containment(min_containment)
+
+    def _device_set_sizes(self):
+        import torch
+        if self._d_set_sizes is None and self._set_sizes is not None:
+            self._d_set_sizes = torch.from_numpy(self._set_sizes).cuda(self.device)
+        return self._d_set_sizes
+
+    def _containment_csr(self, count, fill, items: int, dev, to_host: bool):
+        """count(counts) / dsk_exclusive_scan / fill(iptr, idx, eq, c) over ``items`` (query, partition) items, as ``query``;
+        returns ``(ptr, idx, eq, containment)`` with ptr over the items' queries."""
+        import torch
+        from . import _native as nv
+        counts = torch.empty((max(items, 1),), dtype=torch.int64, device=dev)
+        iptr = torch.empty((items + 1,), dtype=torch.int64, device=dev)
+        scratch = torch.empty((items // 1024 + 2,), dtype=torch.int64, device=dev)
+        st = torch.cuda.current_stream().cuda_stream
+        nv.check(count(counts.data_ptr(), st))
+        nv.check(nv.load().dsk_exclusive_scan(counts.data_ptr(), items, iptr.data_ptr(), scratch.data_ptr(), st))
+        total = int(iptr[items].item())
+        idx = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
+        eq = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
+        c = torch.empty((max(total, 1),), dtype=torch.float64, device=dev)
+        nv.check(fill(iptr.data_ptr(), idx.data_ptr(), eq.data_ptr(), c.data_ptr(), st))
+        out = (iptr[::self.num_part].contiguous(), idx[:total], eq[:total], c[:total])
+        return tuple(x.cpu().numpy() for x in out) if to_host else out
+
+    def query_containment(self, sig, sizes, min_containment: Optional[float] = None, to_host: bool = True):
+        """``query(sig, sizes, with_eq=True)`` with the containment estimate of each candidate, filtered on the device:
+        ``(ptr int64[Q+1], idx int32[M], eq int32[M], containment float64[M])``, each kept candidate once, unordered.
+
+        For query q of size s_q and candidate x of size s_x (its size in the ``index`` call), with ``j = eq / num_perm``
+        (``MinHash.jaccard``), ``c = j * (s_q + s_x) / (s_q * (1 + j))``: the inverse of the map t -> t / (1 + s_x/s_q - t)
+        that the (b, r) table was chosen with, so c estimates |Q & X| / |Q|.  It is the float64 value of that Python
+        expression bit for bit, and it is not clamped: with s_x > s_q and j near 1 it exceeds 1 (``min(c, 1.0)`` caps it).
+        A candidate is kept iff ``c >= min_containment``: ``[x for x in ens.query(m, s) if c(m, s, x) >= t]``.
+        ``min_containment`` is None (keep all, the same as 0.0) or a float in [0, 1]; query sizes are in [1, 2^62);
+        ``ValueError`` otherwise."""
+        import torch
+        from . import _native as nv
+        d_q, sizes, d_qs, d_xs, t = self._containment_args(sig, sizes, min_containment)
+        nq = len(sizes)
+        lib = nv.load()
+        with torch.cuda.device(self.device):
+            sel = torch.from_numpy(self.selection(sizes)).to(d_q.device)
+            args = (self._h, d_q.data_ptr(), nq, d_qs.data_ptr(), sel.data_ptr(), d_xs.data_ptr(), t)
+            return self._containment_csr(
+                lambda counts, st: lib.dsk_lsh_ensemble_containment_count(*args, counts, st),
+                lambda iptr, idx, eq, c, st: lib.dsk_lsh_ensemble_containment_fill(*args, iptr, idx, eq, c, st),
+                nq * self.num_part, d_q.device, to_host)
+
+    def query_topk(self, sig, sizes, k: int, min_containment: Optional[float] = None, to_host: bool = True):
+        """Each query's k (1..32) kept candidates of largest containment estimate: ``(idx int32[Q, k], eq int32[Q, k],
+        containment float64[Q, k])``, in the order ``sorted(kept, key=lambda x: (-c, x))[:k]`` (ties to the smaller row of
+        the ``index`` call), padded with -1 / -1 / -1.0.  Candidates, estimate and filter are ``query_containment``'s.  One
+        kernel launch after the selection table and the sizes are uploaded."""
+        import torch
+        from . import _native as nv
+        from .lsh import _check_topk
+        k = _check_topk(k)
+        d_q, sizes, d_qs, d_xs, t = self._containment_args(sig, sizes, min_containment)
+        nq = len(sizes)
+        dev = d_q.device
+        with torch.cuda.device(self.device):
+            sel = torch.from_numpy(self.selection(sizes)).to(dev)
+            idx = torch.empty((nq, k), dtype=torch.int32, device=dev)
+            eq = torch.empty((nq, k), dtype=torch.int32, device=dev)
+            c = torch.empty((nq, k), dtype=torch.float64, device=dev)
+            nv.check(nv.load().dsk_lsh_ensemble_containment_topk(
+                self._h, d_q.data_ptr(), nq, d_qs.data_ptr(), sel.data_ptr(), d_xs.data_ptr(), t, k, idx.data_ptr(),
+                eq.data_ptr(), c.data_ptr(), torch.cuda.current_stream().cuda_stream))
+        out = (idx, eq, c)
+        return tuple(x.cpu().numpy() for x in out) if to_host else out
+
+    def containment_pairs(self, min_containment: Optional[float] = None, to_host: bool = True):
+        """The self-join: CSR ``(ptr int64[N+1], idx, eq, containment)`` over the rows of the ``index`` call, row i being
+        ``query_containment`` of indexed row i with its own size, without i itself -- the sets that contain at least
+        ``min_containment`` of set i (by the estimate).  Set i is left out by identity: an equal row of equal size is
+        listed.  It reads the index's own rows, so no copy of the signatures is needed.  An index never built gives
+        ``ptr = [0]``."""
+        import torch
+        from . import _native as nv
+        t = _min_containment(min_containment)
+        dev = torch.device("cuda", self.device)
+        if self._set_sizes is None:
+            out = (torch.zeros((1,), dtype=torch.int64, device=dev), torch.zeros((0,), dtype=torch.int32, device=dev),
+                   torch.zeros((0,), dtype=torch.int32, device=dev), torch.zeros((0,), dtype=torch.float64, device=dev))
+            return tuple(x.cpu().numpy() for x in out) if to_host else out
+        lib = nv.load()
+        with torch.cuda.device(self.device):
+            d_xs = self._device_set_sizes()
+            sel = torch.from_numpy(self.selection(self._set_sizes)).to(dev)
+            args = (self._h, sel.data_ptr(), d_xs.data_ptr(), t)
+            return self._containment_csr(
+                lambda counts, st: lib.dsk_lsh_ensemble_self_containment_count(*args, counts, st),
+                lambda iptr, idx, eq, c, st: lib.dsk_lsh_ensemble_self_containment_fill(*args, iptr, idx, eq, c, st),
+                len(self._set_sizes) * self.num_part, dev, to_host)
+
+
+def _min_containment(t) -> float:
+    """``min_containment``: None -> 0.0 (every candidate, c >= 0), else a float in [0, 1]; ``ValueError`` otherwise
+    (NaN included)."""
+    if t is None:
+        return 0.0
+    if isinstance(t, bool) or not isinstance(t, (int, float, np.integer, np.floating)):
+        raise ValueError("min_containment must be None or a float in [0.0, 1.0], got %r" % (t,))
+    t = float(t)
+    if not 0.0 <= t <= 1.0:
+        raise ValueError("min_containment must be in [0.0, 1.0], got %r" % (t,))
+    return t

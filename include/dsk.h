@@ -390,7 +390,31 @@ DSK_API int dsk_lsh_unique_commit(dsk_lsh *ix, const uint32_t *d_sig, int64_t n,
  *                        positions, the number of the num_perm positions where the query row and the set's row agree.
  * Queries check the handle, nq >= 0 and, for nq > 0, every buffer; nq == 0 with null buffers is a valid no-op, and an
  * index that was never built has no candidates.  Cost: one warp per (query, partition) probes b tables of one set and
- * walks the chains it hits, reading the r-tuple of each member (and, with d_eq, both rows of each candidate). */
+ * walks the chains it hits, reading the r-tuple of each member (and, with d_eq, both rows of each candidate).
+ * Containment estimates of the candidates.  For query q of size s_q and candidate x (a row of the index call) of size s_x,
+ * with j = eq / num_perm (MinHash.jaccard): c = j * (s_q + s_x) / (s_q * (1 + j)), the inverse of the map from containment t
+ * to the Jaccard value t / (1 + s_x/s_q - t) that the (b, r) table was chosen for, so c estimates |Q & X| / |Q|.  It is
+ * computed in float64 bit for bit as that Python expression over ints and floats (each operation rounded on its own, s_q + s_x
+ * summed exactly) and not clamped: c exceeds 1 when s_x > s_q and j is near 1.  A candidate is kept iff c >= min_containment
+ * (in [0, 1]; 0 keeps every candidate, since c >= 0).  d_qsizes: int64[nq], each in [1, 2^62); d_set_sizes: int64[n], the
+ * index call's sizes in its row order (the caller keeps them on the device; the index holds its rows in size order only).
+ *   dsk_lsh_ensemble_containment_count  d_counts[q * num_part + p] = the number of kept candidates of q in p (the candidates
+ *                        of dsk_lsh_ensemble_query_count, each with its eq counted when min_containment > 0).
+ *   dsk_lsh_ensemble_containment_fill  after dsk_exclusive_scan of those counts into d_ptr: the kept candidates of each item,
+ *                        each once, unordered, at d_idx[d_ptr[item] ..), with d_eq and d_containment (float64) at the same
+ *                        positions.  With min_containment = 0 the (idx, eq) pairs are those of dsk_lsh_ensemble_query_fill.
+ *   dsk_lsh_ensemble_containment_topk  for each query, its k (1..32) kept candidates of largest c, ties to the smaller row:
+ *                        d_idx / d_eq / d_containment [q * k .. q * k + k), padded with -1 / -1 / -1.0.  One launch, no
+ *                        scan: one warp per query walks its partitions in turn and keeps a warp-held list.
+ *   dsk_lsh_ensemble_self_containment_count / _fill  the self-join: the same for each indexed set i as a query (its own row
+ *                        and size d_set_sizes[i]), set i itself left out by identity (an equal row of equal size is still
+ *                        listed).  d_sel is [n, num_part] in the index call's row order (built from the indexed sizes), the
+ *                        items are i * num_part + p in that order, and nothing is read but the index's own rows.  An index
+ *                        never built is a no-op.
+ * Each returns DSK_ERR_INVALID with a message for a null handle, nq < 0, a null buffer when there is work (nq > 0, or n > 0
+ * for the self-join), k outside [1, 32], and min_containment NaN or outside [0, 1]; nq == 0 with null buffers is a no-op.
+ * Cost: the walk of the query functions, plus one K-word row comparison per candidate (the count pass skips it when
+ * min_containment is 0) and one int64 size read. */
 typedef struct dsk_lsh_ensemble dsk_lsh_ensemble;
 DSK_API int dsk_lsh_ensemble_create(int num_perm, int num_part, const int32_t *h_b, const int32_t *h_r, int n_params,
                                     int device, dsk_lsh_ensemble **out);
@@ -403,6 +427,22 @@ DSK_API int dsk_lsh_ensemble_query_count(const dsk_lsh_ensemble *e, const uint32
                                          int64_t *d_counts, void *stream);
 DSK_API int dsk_lsh_ensemble_query_fill(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq, const int32_t *d_sel,
                                         const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq, void *stream);
+DSK_API int dsk_lsh_ensemble_containment_count(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq,
+                                               const int64_t *d_qsizes, const int32_t *d_sel, const int64_t *d_set_sizes,
+                                               double min_containment, int64_t *d_counts, void *stream);
+DSK_API int dsk_lsh_ensemble_containment_fill(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq,
+                                              const int64_t *d_qsizes, const int32_t *d_sel, const int64_t *d_set_sizes,
+                                              double min_containment, const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq,
+                                              double *d_containment, void *stream);
+DSK_API int dsk_lsh_ensemble_containment_topk(const dsk_lsh_ensemble *e, const uint32_t *d_qsig, int64_t nq,
+                                              const int64_t *d_qsizes, const int32_t *d_sel, const int64_t *d_set_sizes,
+                                              double min_containment, int k, int32_t *d_idx, int32_t *d_eq,
+                                              double *d_containment, void *stream);
+DSK_API int dsk_lsh_ensemble_self_containment_count(const dsk_lsh_ensemble *e, const int32_t *d_sel, const int64_t *d_set_sizes,
+                                                    double min_containment, int64_t *d_counts, void *stream);
+DSK_API int dsk_lsh_ensemble_self_containment_fill(const dsk_lsh_ensemble *e, const int32_t *d_sel, const int64_t *d_set_sizes,
+                                                   double min_containment, const int64_t *d_ptr, int32_t *d_idx, int32_t *d_eq,
+                                                   double *d_containment, void *stream);
 /* The size partitions of MinHashLSHEnsemble.index (lshensemble_partition.py:54-196, optimal_partitions), on the device.
  * h_sizes / h_counts (host memory, n_sizes = D entries): the distinct set sizes, strictly ascending, and their counts, every
  * value in [1, 2^62).  Writes h_upper_idx[k] (host memory, min(num_part, D) entries) = the index into h_sizes of the upper
