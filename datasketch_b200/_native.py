@@ -50,6 +50,8 @@ SIGNATURES = {
     "dsk_wmh_create": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
     "dsk_wmh_destroy": (None, [c_void_p]),
     "dsk_wmh_minhash": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p]),
+    "dsk_wmh_minhash_csr": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int,
+                                    c_void_p]),
     "dsk_lsh_create": (c_int, [c_int, c_int, c_int, c_int64, c_int, ctypes.POINTER(c_void_p)]),
     "dsk_lsh_create_weighted": (c_int, [c_int, c_int, c_int, c_int64, c_int, ctypes.POINTER(c_void_p)]),
     "dsk_lsh_destroy": (None, [c_void_p]),

@@ -716,6 +716,24 @@ int dsk_wmh_minhash(const dsk_wmh *g, const float *d_v, int64_t n, int64_t *d_ou
     return DSK_OK;
 }
 
+int dsk_wmh_minhash_csr(const dsk_wmh *g, const int64_t *d_indptr, const int32_t *d_indices, const float *d_vals, int64_t n,
+                        int64_t *d_out, int32_t *d_status, int flags, void *stream) {
+    if (!g || n < 0 || (flags & ~(DSK_WMH_MINHASH_MANY | DSK_WMH_INPUT_LOG)) != 0 ||
+        (n > 0 && (!d_indptr || !d_indices || !d_vals || !d_out || !d_status))) {
+        set_error("dsk_wmh_minhash_csr: bad arguments");
+        return DSK_ERR_INVALID;
+    }
+    DevInfo *dev;
+    int rc = get_dev(g->device, &dev);
+    if (rc) return rc;
+    const size_t plane = (size_t)g->dim * g->ss_pad;
+    DevGuard guard(g->device);
+    DSK_CUDA(launch_wmh_csr(g->d_par, g->d_par + plane, g->d_par + 2 * plane, g->ss, g->ss_pad, g->dim, d_indptr, d_indices,
+                            d_vals, n, d_out, d_status, (flags & DSK_WMH_MINHASH_MANY) != 0,
+                            (flags & DSK_WMH_INPUT_LOG) != 0, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
 // num_perm samples of sw words each; b and r count samples
 static int lsh_create(const char *who, int num_perm, int sw, int b, int r, int64_t capacity_docs, int device, dsk_lsh **out) {
     int rc = check_bands(who, capacity_docs, num_perm, b, r);

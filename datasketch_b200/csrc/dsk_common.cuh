@@ -123,6 +123,9 @@ cudaError_t launch_wmh_transpose(const float *src, int ss, int dim, int ss_pad, 
 cudaError_t launch_wmh(const float *rs_t, const float *lncs_t, const float *betas_t, int ss, int ss_pad, int dim,
                        const float *v, int64_t n, int64_t *out, int32_t *status, int many, int input_log, int sm_count,
                        cudaStream_t s);
+cudaError_t launch_wmh_csr(const float *rs_t, const float *lncs_t, const float *betas_t, int ss, int ss_pad, int dim,
+                           const int64_t *indptr, const int32_t *indices, const float *vals, int64_t n, int64_t *out,
+                           int32_t *status, int many, int input_log, int sm_count, cudaStream_t s);
 
 // ---- device-resident LSH index (lsh_kernels.cu) -------------------------------------------------
 struct LshDev {

@@ -159,6 +159,112 @@ __global__ void __launch_bounds__(kWmhThreads) wmh_kernel(const WmhParams p) {
     }
 }
 
+// ---- sparse rows (CSR) ---------------------------------------------------------------------------------------------
+// The same evaluation over a row's stored entries only, in ascending column order.  A left-out column is a zero
+// weight, whose ln_a = +inf never wins, and the comparison is strict over ascending columns, so the result equals
+// wmh_kernel on the densified row.  No parameter is reused across rows here: each entry costs its three parameter
+// loads (12 B per sample, from L2 or HBM), so the kernel is bound by that gather, not by the evaluation.
+constexpr int kCsrTile = 512;    // entries staged per tile
+constexpr int kCsrUnroll = 8;    // entries whose parameter loads are in flight together
+
+struct WmhCsrParams {
+    const float *rs_t, *lncs_t, *betas_t;  // [dim][ss_pad]
+    int ss, ss_pad, dim;
+    const int64_t *indptr;                 // [n + 1], starts at 0, non-decreasing
+    const int32_t *indices;                // [nnz] column of each entry
+    const float *vals;                     // [nnz] weight, or ln(weight) with input_log
+    int64_t n;
+    int64_t *out;                          // [n][ss][2]
+    int32_t *status;                       // [n]: as WmhParams, and 3 = columns not strictly increasing or outside [0, dim)
+    int input_log;
+};
+
+template <bool MANY>
+__global__ void __launch_bounds__(kWmhThreads) wmh_csr_kernel(const WmhCsrParams p) {
+    // padded to a whole trip of kCsrUnroll: padding is column 0 with vlog = -inf, which never wins
+    __shared__ int s_col[kCsrTile];
+    __shared__ float s_vlog[kCsrTile];
+    __shared__ int64_t s_bad_row;          // the last row found malformed
+    const int tid = threadIdx.x;
+    const int s = blockIdx.y * kWmhThreads + tid;
+    const bool s_ok = s < p.ss;
+    if (tid == 0) s_bad_row = -1;
+
+    for (int64_t row = blockIdx.x; row < p.n; row += gridDim.x) {
+        const int64_t e0 = p.indptr[row], e1 = p.indptr[row + 1];
+        float best = __int_as_float(0x7f800000), bt = 0.f;
+        int bk = -1;
+        bool bad = false;
+        for (int64_t t0 = e0; t0 < e1 && !bad; t0 += kCsrTile) {
+            const int ne = (int)min((int64_t)kCsrTile, e1 - t0);
+            const int ne_pad = (ne + kCsrUnroll - 1) / kCsrUnroll * kCsrUnroll;
+            __syncthreads();  // previous tile fully consumed (and s_bad_row initialised)
+            for (int i = tid; i < ne_pad; i += kWmhThreads) {
+                int c = 0;
+                float lg = __int_as_float(0xff800000);
+                if (i < ne) {
+                    const int64_t e = t0 + i;
+                    const int col = __ldg(p.indices + e);
+                    const int prev = e > e0 ? __ldg(p.indices + e - 1) : -1;
+                    if (col <= prev || col >= p.dim) s_bad_row = row;   // col < 0 implies col <= prev
+                    else c = col;
+                    const float x = __ldg(p.vals + e);
+                    lg = p.input_log ? x : (float)log((double)x);
+                }
+                s_col[i] = c;
+                s_vlog[i] = lg;
+            }
+            __syncthreads();
+            bad = s_bad_row == row;
+            if (bad || !s_ok) continue;
+            for (int i = 0; i < ne_pad; i += kCsrUnroll) {
+                float r[kCsrUnroll], lc[kCsrUnroll], be[kCsrUnroll];
+#pragma unroll
+                for (int q = 0; q < kCsrUnroll; ++q) {
+                    const int64_t off = (int64_t)s_col[i + q] * p.ss_pad + s;   // passes 2^31 at dim 2^24
+                    r[q] = __ldg(p.rs_t + off);
+                    lc[q] = __ldg(p.lncs_t + off);
+                    be[q] = __ldg(p.betas_t + off);
+                }
+#pragma unroll
+                for (int q = 0; q < kCsrUnroll; ++q) {
+                    const float t = floorf(__fadd_rn(__fdiv_rn(s_vlog[i + q], r[q]), be[q]));
+                    const float ln_a = wmh_ln_a<MANY>(t, be[q], r[q], lc[q]);
+                    if (wmh_better<MANY>(ln_a, best)) {
+                        best = ln_a; bk = s_col[i + q]; bt = t;
+                    }
+                }
+            }
+        }
+        if (s_ok) {
+            int64_t *o = p.out + (row * p.ss + s) * 2;
+            const bool fin = isfinite(bt);
+            o[0] = bad || bk < 0 ? 0 : bk;
+            o[1] = bad || bk < 0 ? 0 : fin ? (int64_t)bt : INT64_MIN;
+            if (s == 0) p.status[row] = bad ? 3 : bk < 0 ? 1 : fin ? 0 : 2;
+        }
+    }
+}
+
+cudaError_t launch_wmh_csr(const float *rs_t, const float *lncs_t, const float *betas_t, int ss, int ss_pad, int dim,
+                           const int64_t *indptr, const int32_t *indices, const float *vals, int64_t n, int64_t *out,
+                           int32_t *status, int many, int input_log, int sm_count, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    WmhCsrParams p;
+    p.rs_t = rs_t; p.lncs_t = lncs_t; p.betas_t = betas_t;
+    p.ss = ss; p.ss_pad = ss_pad; p.dim = dim;
+    p.indptr = indptr; p.indices = indices; p.vals = vals;
+    p.n = n; p.out = out; p.status = status; p.input_log = input_log;
+    const int slices = (ss + kWmhThreads - 1) / kWmhThreads;
+    int64_t gx = n;
+    const int64_t cap = (int64_t)sm_count * 16;   // 16 CTAs of 128 threads fill an SM's 2,048 threads
+    if (gx > cap) gx = cap;
+    dim3 grid((unsigned)gx, (unsigned)slices);
+    if (many) DSK_LAUNCH((wmh_csr_kernel<true>), grid, kWmhThreads, 0, s, p);
+    else DSK_LAUNCH((wmh_csr_kernel<false>), grid, kWmhThreads, 0, s, p);
+    return cudaGetLastError();
+}
+
 // [ss][dim] -> [dim][ss_pad] (one-time, at generator creation)
 __global__ void wmh_transpose_kernel(const float *src, int ss, int dim, int ss_pad, float *dst) {
     const int64_t total = (int64_t)dim * ss_pad, stride = (int64_t)gridDim.x * blockDim.x;

@@ -3,7 +3,9 @@
 ``WeightedMinHashGenerator.__init__`` draws the ICWS parameters on the host with numpy,
 bit-identically to the reference (:118-121).  ``minhash`` (one vector) and
 ``minhash_batch`` (a matrix) run the per-sample argmin in ``libdsk_b200.so``
-(``dsk_wmh_minhash``); every float32 step after ``log`` is IEEE-identical to numpy.
+(``dsk_wmh_minhash``); every float32 step after ``log`` is IEEE-identical to numpy.  Sparse matrices
+(scipy.sparse, CUDA ``torch.sparse_csr``) go to ``dsk_wmh_minhash_csr`` as their stored entries, with the results of
+their densified rows.
 """
 from __future__ import annotations
 
@@ -48,6 +50,52 @@ class WeightedMinHash:
                 and np.array_equal(self.hashvalues, other.hashvalues))
 
     __hash__ = None
+
+
+def _is_sparse(X) -> bool:
+    """A scipy.sparse matrix or array, or a torch tensor in the sparse CSR layout."""
+    if hasattr(X, "tocsr") and hasattr(X, "nnz"):
+        return True
+    layout = getattr(X, "layout", None)
+    return layout is not None and str(layout) == "torch.sparse_csr"
+
+
+def _csr_arrays(X, dim: int):
+    """A scipy.sparse matrix -> (indptr int64 [n + 1], indices int32 [nnz], weights float32 [nnz]) in canonical CSR
+    form, whose rows densify to exactly ``np.asarray(X.tocsr().toarray(), dtype=np.float32)``.
+
+    ``toarray()`` sums duplicate entries in the matrix's own dtype, in stored order, starting from 0; in float32
+    ``1 + 1e8 - 1e8`` is 0 but ``1e8 - 1e8 + 1`` is 1, so the order matters.  A stable sort by column within each row
+    keeps that order and ``np.add.at`` adds in it (``sum_duplicates()`` sorts unstably).  The cast to float32 follows
+    the sums, as it follows ``toarray()``."""
+    X = X.tocsr()
+    if X.ndim != 2 or X.shape[1] != dim:
+        raise ValueError("Input dimension mismatch, expecting %d" % dim)
+    n = X.shape[0]
+    indptr = np.asarray(X.indptr, dtype=np.int64)
+    indices, data = np.asarray(X.indices), np.asarray(X.data)
+    if (len(indptr) != n + 1 or indptr[0] != 0 or bool((indptr[1:] < indptr[:-1]).any())
+            or indptr[-1] > min(len(indices), len(data))):
+        raise ValueError("the matrix's indptr must start at 0, be non-decreasing and end at most at nnz")
+    nnz = int(indptr[-1])
+    indices, data = indices[:nnz], data[:nnz]
+    if nnz and (int(indices.min()) < 0 or int(indices.max()) >= dim):
+        bad = (indices < 0) | (indices >= dim)
+        raise ValueError("row %d: column indices fall outside [0, %d)"
+                         % (int(np.searchsorted(indptr, np.argmax(bad), side="right")) - 1, dim))
+    if not X.has_canonical_format:
+        key = np.repeat(np.arange(n, dtype=np.int64), np.diff(indptr)) * dim + indices.astype(np.int64)
+        order = np.argsort(key, kind="stable")
+        key = key[order]
+        first = np.ones(len(key), dtype=bool)
+        first[1:] = key[1:] != key[:-1]
+        summed = np.zeros(int(first.sum()), dtype=data.dtype)
+        np.add.at(summed, np.cumsum(first) - 1, data[order])
+        key, data = key[first], summed
+        indices = key % dim
+        indptr = np.zeros(n + 1, dtype=np.int64)
+        np.cumsum(np.bincount(key // dim, minlength=n), out=indptr[1:])
+    return indptr, indices.astype(np.int32, copy=False), data.astype(np.float32, copy=False)
 
 
 class WeightedMinHashGenerator:
@@ -132,6 +180,55 @@ class WeightedMinHashGenerator:
             return d_out, d_st
         return d_out.cpu().numpy(), d_st.cpu().numpy()
 
+    def _sample_csr(self, X, device: int, many: bool, device_log: bool = False, to_host: bool = True):
+        """``_sample`` for sparse rows through ``dsk_wmh_minhash_csr``: a scipy.sparse matrix (prepared on the host by
+        :func:`_csr_arrays`; host logarithm unless ``device_log``) or a CUDA ``torch.sparse_csr`` tensor (device
+        logarithm).  Status 3 marks a row whose columns are not strictly increasing or fall outside [0, dim)."""
+        import torch
+        flags = int(many)
+        if isinstance(X, torch.Tensor):
+            if X.dim() != 2 or X.shape[1] != self.dim:
+                raise ValueError("Input dimension mismatch, expecting %d" % self.dim)
+            if not X.is_cuda:
+                raise ValueError("a torch.sparse_csr input must be a CUDA tensor")
+            dev = X.device
+            n = X.shape[0]
+            indptr = X.crow_indices().to(torch.int64)
+            cols = X.col_indices()
+            if len(indptr) != n + 1 or bool(((indptr[0] != 0) | (indptr[-1] > len(cols))
+                                             | (indptr[1:] < indptr[:-1]).any()).item()):
+                raise ValueError("crow_indices must start at 0, be non-decreasing and end at most at nnz")
+            # out-of-range columns become -1 or dim, which the kernel reports as status 3 (a plain int32 cast could wrap)
+            cols = cols.clamp(-1, self.dim).to(torch.int32).contiguous()
+            vals = X.values().to(torch.float32).contiguous()
+        else:
+            indptr, cols, vals = _csr_arrays(X, self.dim)
+            n = len(indptr) - 1
+            if not device_log:
+                with np.errstate(invalid="ignore", divide="ignore"):
+                    vals = np.log(vals)      # numpy's float32 log of the stored values, as the dense path takes it
+                flags |= 2   # DSK_WMH_INPUT_LOG
+            dev = torch.device("cuda", device)
+            indptr, cols, vals = (torch.from_numpy(a).to(dev) for a in (indptr, cols, vals))
+        if len(cols) == 0:                   # the kernel reads no entry, but its buffers must not be NULL
+            cols = torch.zeros(1, dtype=torch.int32, device=dev)
+            vals = torch.zeros(1, dtype=torch.float32, device=dev)
+        h = self._handle(dev.index)
+        d_out = torch.empty((n, self.sample_size, 2), dtype=torch.int64, device=dev)
+        d_st = torch.empty((n,), dtype=torch.int32, device=dev)
+        if n:
+            with torch.cuda.device(dev):
+                nv.check(nv.load().dsk_wmh_minhash_csr(h, indptr.data_ptr(), cols.data_ptr(), vals.data_ptr(), n,
+                                                       d_out.data_ptr(), d_st.data_ptr(), flags,
+                                                       torch.cuda.current_stream(dev).cuda_stream))
+        bad = d_st == 3
+        if n and bool(bad.any()):
+            raise ValueError("row %d: column indices are not strictly increasing or fall outside [0, %d)"
+                             % (int(bad.nonzero()[0][0]), self.dim))
+        if not to_host:
+            return d_out, d_st
+        return d_out.cpu().numpy(), d_st.cpu().numpy()
+
     @staticmethod
     def _raise_status(status, empty_message: str) -> None:
         worst = int(status.max()) if len(status) else 0
@@ -144,8 +241,15 @@ class WeightedMinHashGenerator:
         """[n, dim] weights -> [n, sample_size, 2] int64 of (k, t) -- row i equals
         ``self.minhash(X[i]).hashvalues``.  Raises ValueError if a row has no positive weight and OverflowError if
         one holds +inf.  ``to_host=False`` returns the CUDA int64 tensor (the same values), which
-        ``GpuLSH(weighted=True)`` takes as it is: weights -> signatures -> index without a copy to the host."""
-        out, status = self._sample(X, device, many=False, device_log=device_log, to_host=to_host)
+        ``GpuLSH(weighted=True)`` takes as it is: weights -> signatures -> index without a copy to the host.
+
+        ``X`` may be sparse: a scipy.sparse matrix (row i equals ``minhash(X[i].toarray().ravel())``, with the host
+        logarithm) or a CUDA ``torch.sparse_csr`` tensor (equal to ``minhash_batch(X.to_dense())``, with the device
+        logarithm).  Sparse rows are sampled over their stored entries only, never densified."""
+        if _is_sparse(X):
+            out, status = self._sample_csr(X, device, many=False, device_log=device_log, to_host=to_host)
+        else:
+            out, status = self._sample(X, device, many=False, device_log=device_log, to_host=to_host)
         self._raise_status(status, "Input is all zeros")
         return out
 
@@ -172,8 +276,9 @@ class WeightedMinHashGenerator:
         The reference's experimental method rounds ``ln_a`` in a different order than ``minhash``
         (:221-224: ``ln_y = (t - beta + 1) * r; ln_a = ln_c - ln_y``); the kernel's
         ``DSK_WMH_MINHASH_MANY`` mode follows that order, so the values are the reference's
-        ``minhash_many`` values, not necessarily ``minhash``'s.  Rows go to the device densified, in
-        slabs of at most 256 MB."""
+        ``minhash_many`` values, not necessarily ``minhash``'s.  A numpy matrix goes to the device in
+        slabs of at most 256 MB; a scipy.sparse matrix goes as its stored entries (``dsk_wmh_minhash_csr``),
+        with the same results as its densified rows."""
         sparse = hasattr(X, "tocsr") and hasattr(X, "nnz")
         if not sparse and not isinstance(X, np.ndarray):
             raise TypeError("Input X must be a sparse matrix or numpy matrix")
@@ -181,14 +286,18 @@ class WeightedMinHashGenerator:
             raise ValueError("Input must have two dimensions")
         if X.shape[1] != self.dim:
             raise ValueError("Input dimension mismatch, expecting %d" % self.dim)
-        if sparse:
-            X = X.tocsr()
         n = X.shape[0]
         ret: List[Optional[WeightedMinHash]] = [None] * n
+        if sparse:
+            out, status = self._sample_csr(X, device, many=True)
+            for i in range(n):
+                if status[i] != 1:
+                    ret[i] = WeightedMinHash(self.seed, out[i].astype(int, copy=False))
+            return ret
         slab = max(1, (256 << 20) // (4 * max(self.dim, 1)))
         for r0 in range(0, n, slab):
             part = X[r0:r0 + slab]
-            dense = np.asarray(part.toarray() if sparse else part, dtype=np.float32)
+            dense = np.asarray(part, dtype=np.float32)
             out, status = self._sample(dense, device, many=True)
             for i in range(out.shape[0]):
                 if status[i] != 1:

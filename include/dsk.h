@@ -223,6 +223,18 @@ DSK_API int dsk_wmh_create(const float *h_rs, const float *h_ln_cs, const float 
 DSK_API void dsk_wmh_destroy(dsk_wmh *g);
 DSK_API int dsk_wmh_minhash(const dsk_wmh *g, const float *d_v, int64_t n, int64_t *d_out, int32_t *d_status,
                             int flags, void *stream);
+/* dsk_wmh_minhash_csr: the same sampling for n SPARSE rows in CSR form, in time linear in their stored entries (the
+ * sparse path of the reference's minhash_many, :191-239, without densifying).  Row i holds the entries
+ * [d_indptr[i], d_indptr[i + 1]) of d_indices (column) and d_vals (weight, or ln(weight) with DSK_WMH_INPUT_LOG).
+ *   d_indptr  [n + 1] int64: must start at 0 and be non-decreasing (not checked here: the kernel reads the entries it
+ *             names; the host layer checks it before the call)
+ *   d_indices [nnz] int32: strictly increasing within each row, each in [0, dim); a row that breaks this gets status 3
+ *             and (0, 0) in every sample, and is not evaluated further
+ *   d_out, d_status, flags: as dsk_wmh_minhash.  Each row's result equals dsk_wmh_minhash on the densified row bit for
+ *             bit: a left-out column is a zero weight, which never wins, and explicit zeros may be stored.
+ * n == 0 is a no-op (the buffers may then be NULL); for n > 0 every pointer must be non-NULL. */
+DSK_API int dsk_wmh_minhash_csr(const dsk_wmh *g, const int64_t *d_indptr, const int32_t *d_indices, const float *d_vals,
+                                int64_t n, int64_t *d_out, int32_t *d_status, int flags, void *stream);
 
 /* ---- device-resident MinHashLSH index ------------------------------------------------------
  * Replaces the bucket step of MinHashLSH._insert / query over dict storage
