@@ -18,7 +18,7 @@ from .lsh import GpuLSH, MinHashLSH, MinHashLSHDeletionSession, MinHashLSHInsert
 from .lshforest import GpuLSHForest, MinHashLSHForest  # noqa: E402
 from .lshensemble import GpuLSHEnsemble, MinHashLSHEnsemble  # noqa: E402
 from .lsh_bloom import MinHashLSHBloom  # noqa: E402
-from . import codec, distributed, engine  # noqa: E402
+from . import codec, distributed, engine, shingle  # noqa: E402
 
 # aliases kept by the reference (datasketch/__init__.py)
 WeightedMinHashLSH = MinHashLSH
@@ -26,4 +26,4 @@ WeightedMinHashLSHForest = MinHashLSHForest
 
 __version__ = "0.1.0"
 __all__ = ["MinHash", "LeanMinHash", "bBitMinHash", "WeightedMinHash", "WeightedMinHashGenerator", "MinHashLSH", "GpuLSH", "MinHashLSHForest", "GpuLSHForest", "MinHashLSHEnsemble", "GpuLSHEnsemble", "MinHashLSHBloom", "MinHashLSHBloom",
-           "WeightedMinHashLSH", "WeightedMinHashLSHForest", "MinHashLSHInsertionSession", "MinHashLSHDeletionSession", "sha1_hash32", "sha1_hash64", "xxh32_hash32", "murmur3_hash32", "engine", "codec", "distributed"]
+           "WeightedMinHashLSH", "WeightedMinHashLSHForest", "MinHashLSHInsertionSession", "MinHashLSHDeletionSession", "sha1_hash32", "sha1_hash64", "xxh32_hash32", "murmur3_hash32", "engine", "codec", "distributed", "shingle"]

@@ -103,6 +103,11 @@ SIGNATURES = {
                                     ctypes.c_size_t, c_void_p]),
     "dsk_sha1_tokens": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int, c_void_p]),
     "dsk_hash_tokens": (c_int, [c_void_p, c_void_p, c_int64, c_int, ctypes.c_uint32, c_void_p, c_void_p]),
+    "dsk_shingle_workspace_size": (c_size_t, [c_int64, c_int64]),
+    "dsk_shingle_count": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t,
+                                  c_void_p]),
+    "dsk_shingle_hash": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_int, ctypes.c_uint32, c_void_p,
+                                 c_void_p, c_void_p, c_size_t, c_void_p]),
     "dsk_bbit_pack": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),
     "dsk_bbit_unpack": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),
     "dsk_forest_query": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_int, c_void_p,

@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "dsk_common.cuh"
+#include "shingle_kernels.cuh"   // the shingle kernels are compiled here, beside their entry points
 
 namespace dsk {
 
@@ -1745,6 +1746,82 @@ int dsk_hash_tokens(const uint8_t *d_bytes, const int64_t *d_byte_offsets, int64
     int rc = current_dev(&dev);
     if (rc) return rc;
     DSK_CUDA(launch_hash_tokens(d_bytes, d_byte_offsets, n_tokens, kind, seed, d_out, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+size_t dsk_shingle_workspace_size(int64_t n_docs, int64_t n_bytes) {
+    return n_docs < 0 || n_bytes < 0 ? 0 : shingle_workspace_bytes(n_docs, n_bytes);
+}
+
+static int check_shingle(const char *who, const uint8_t *d_text, const int64_t *d_doc_offsets, int64_t n_docs,
+                         int64_t n_bytes, int unit, int n, const void *d_ws, size_t ws_bytes) {
+    if (n_docs < 0 || n_bytes < 0 || n < 1 || (unit != DSK_SHINGLE_WORD && unit != DSK_SHINGLE_CHAR) || !d_doc_offsets ||
+        (n_bytes > 0 && !d_text)) {
+        set_error("%s: bad arguments (n_docs, n_bytes >= 0, n >= 1, unit DSK_SHINGLE_WORD or DSK_SHINGLE_CHAR)", who);
+        return DSK_ERR_INVALID;
+    }
+    const size_t need = shingle_workspace_bytes(n_docs, n_bytes);
+    if (!d_ws || ((uintptr_t)d_ws & 15) != 0 || ws_bytes < need) {
+        set_error("%s: the workspace must be 16-byte aligned and hold dsk_shingle_workspace_size() = %zu bytes (got %zu)", who,
+                  need, ws_bytes);
+        return DSK_ERR_INVALID;
+    }
+    if (((uintptr_t)d_doc_offsets & 7) != 0) {
+        set_error("%s: d_doc_offsets must be 8-byte aligned", who);
+        return DSK_ERR_ALIGN;
+    }
+    return DSK_OK;
+}
+
+int dsk_shingle_count(const uint8_t *d_text, const int64_t *d_doc_offsets, int64_t n_docs, int64_t n_bytes, int unit, int n,
+                      int64_t *d_tok_offsets, int32_t *d_doc_status, void *d_ws, size_t ws_bytes, void *stream) {
+    int rc = check_shingle("dsk_shingle_count", d_text, d_doc_offsets, n_docs, n_bytes, unit, n, d_ws, ws_bytes);
+    if (rc) return rc;
+    if (!d_tok_offsets || !d_doc_status) {
+        set_error("dsk_shingle_count: null output");
+        return DSK_ERR_INVALID;
+    }
+    if (((uintptr_t)d_tok_offsets & 7) != 0 || ((uintptr_t)d_doc_status & 3) != 0) {
+        set_error("dsk_shingle_count: d_tok_offsets must be 8-byte and d_doc_status 4-byte aligned");
+        return DSK_ERR_ALIGN;
+    }
+    if (n_docs == 0) {   // no document: no byte is read
+        DSK_CUDA(cudaMemsetAsync(d_tok_offsets, 0, sizeof(int64_t), (cudaStream_t)stream));
+        DSK_CUDA(cudaMemsetAsync(d_doc_status, 0, sizeof(int32_t), (cudaStream_t)stream));
+        return DSK_OK;
+    }
+    DevInfo *dev;
+    rc = current_dev(&dev);
+    if (rc) return rc;
+    DSK_CUDA(shingle_count(d_text, d_doc_offsets, n_docs, n_bytes, unit == DSK_SHINGLE_WORD, n, d_tok_offsets, d_doc_status,
+                           d_ws, dev->sm_count, (cudaStream_t)stream));
+    return DSK_OK;
+}
+
+int dsk_shingle_hash(const uint8_t *d_text, const int64_t *d_doc_offsets, int64_t n_docs, int64_t n_bytes, int unit, int n,
+                     int hash_kind, uint32_t seed, const int64_t *d_tok_offsets, uint32_t *d_tokens, void *d_ws,
+                     size_t ws_bytes, void *stream) {
+    int rc = check_shingle("dsk_shingle_hash", d_text, d_doc_offsets, n_docs, n_bytes, unit, n, d_ws, ws_bytes);
+    if (rc) return rc;
+    if (hash_kind != 0 && hash_kind != DSK_HASH_XXH32 && hash_kind != DSK_HASH_MURMUR3_32) {
+        set_error("dsk_shingle_hash: hash_kind must be 0 (sha1_hash32), DSK_HASH_XXH32 or DSK_HASH_MURMUR3_32 (got %d)",
+                  hash_kind);
+        return DSK_ERR_INVALID;
+    }
+    if (!d_tok_offsets || !d_tokens) {
+        set_error("dsk_shingle_hash: null buffer");
+        return DSK_ERR_INVALID;
+    }
+    if (((uintptr_t)d_tok_offsets & 7) != 0 || ((uintptr_t)d_tokens & 3) != 0) {
+        set_error("dsk_shingle_hash: d_tok_offsets must be 8-byte and d_tokens 4-byte aligned");
+        return DSK_ERR_ALIGN;
+    }
+    if (n_docs == 0) return DSK_OK;
+    DevInfo *dev;
+    rc = current_dev(&dev);
+    if (rc) return rc;
+    DSK_CUDA(shingle_hash(d_text, d_doc_offsets, n_docs, n_bytes, unit == DSK_SHINGLE_WORD, n, hash_kind, seed, d_tok_offsets,
+                          d_tokens, d_ws, dev->sm_count, (cudaStream_t)stream));
     return DSK_OK;
 }
 

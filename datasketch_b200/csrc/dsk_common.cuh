@@ -230,6 +230,13 @@ cudaError_t launch_sha1_tokens(const uint8_t *bytes, const int64_t *off, int64_t
                                int sm_count, cudaStream_t s);
 cudaError_t launch_hash_tokens(const uint8_t *bytes, const int64_t *off, int64_t n_tok, int kind, uint32_t seed,
                                uint32_t *out, int sm_count, cudaStream_t s);
+// raw UTF-8 text -> word / character n-gram tokens (shingle_kernels.cuh, DESIGN.md §4m): the workspace both passes share,
+// the count pass (offsets check, per-document status, token offsets) and the hash pass (one u32 token per shingle)
+size_t shingle_workspace_bytes(int64_t n_docs, int64_t n_bytes);
+cudaError_t shingle_count(const uint8_t *text, const int64_t *off, int64_t n_docs, int64_t n_bytes, int word, int n,
+                          int64_t *tok_off, int32_t *status, void *ws, int sm_count, cudaStream_t s);
+cudaError_t shingle_hash(const uint8_t *text, const int64_t *off, int64_t n_docs, int64_t n_bytes, int word, int n, int kind,
+                         uint32_t seed, const int64_t *tok_off, uint32_t *out, void *ws, int sm_count, cudaStream_t s);
 
 cudaError_t launch_bbit_pack(const uint32_t *sig, int64_t n, int k, int b, int slot, uint64_t *out, int sm_count,
                              cudaStream_t s);

@@ -4,63 +4,11 @@
 // `mmh3.hash(d, signed=False)`, `xxhash`).  Both algorithms live in third-party packages, not in the reference's tree:
 //   XXH32            -- xxHash specification (Y. Collet), 32-bit variant; pinned against the `xxhash` package
 //   MurmurHash3 x86_32 -- A. Appleby's public-domain MurmurHash3; pinned against its published vectors
-// thread <-> token; words are assembled from bytes (tokens start at arbitrary byte offsets of the blob).
-#include "dsk_common.cuh"
+// thread <-> token; words are assembled from bytes (tokens start at arbitrary byte offsets of the blob).  The cores are
+// xxh32 / murmur3_32 in hash_core.cuh, shared with the shingle kernels.
+#include "hash_core.cuh"
 
 namespace dsk {
-
-namespace {
-__device__ __forceinline__ uint32_t rotl(uint32_t x, int n) { return (x << n) | (x >> (32 - n)); }
-__device__ __forceinline__ uint32_t le32(const uint8_t *__restrict__ p) {
-    return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
-}
-
-__device__ __forceinline__ uint32_t xxh32(const uint8_t *__restrict__ d, int64_t len, uint32_t seed) {
-    constexpr uint32_t P1 = 2654435761u, P2 = 2246822519u, P3 = 3266489917u, P4 = 668265263u, P5 = 374761393u;
-    int64_t i = 0;
-    uint32_t h;
-    if (len >= 16) {
-        uint32_t v1 = seed + P1 + P2, v2 = seed + P2, v3 = seed, v4 = seed - P1;
-        for (; i + 16 <= len; i += 16) {
-            v1 = rotl(v1 + le32(d + i) * P2, 13) * P1;
-            v2 = rotl(v2 + le32(d + i + 4) * P2, 13) * P1;
-            v3 = rotl(v3 + le32(d + i + 8) * P2, 13) * P1;
-            v4 = rotl(v4 + le32(d + i + 12) * P2, 13) * P1;
-        }
-        h = rotl(v1, 1) + rotl(v2, 7) + rotl(v3, 12) + rotl(v4, 18);
-    } else {
-        h = seed + P5;
-    }
-    h += (uint32_t)len;
-    for (; i + 4 <= len; i += 4) h = rotl(h + le32(d + i) * P3, 17) * P4;
-    for (; i < len; ++i) h = rotl(h + (uint32_t)d[i] * P5, 11) * P1;
-    h ^= h >> 15; h *= P2; h ^= h >> 13; h *= P3; h ^= h >> 16;
-    return h;
-}
-
-__device__ __forceinline__ uint32_t murmur3_32(const uint8_t *__restrict__ d, int64_t len, uint32_t seed) {
-    constexpr uint32_t C1 = 0xcc9e2d51u, C2 = 0x1b873593u;
-    uint32_t h = seed;
-    int64_t i = 0;
-    for (; i + 4 <= len; i += 4) {
-        uint32_t k = le32(d + i) * C1;
-        k = rotl(k, 15) * C2;
-        h = rotl(h ^ k, 13) * 5u + 0xe6546b64u;
-    }
-    uint32_t k = 0;
-    const int tail = (int)(len - i);
-    if (tail == 3) k ^= (uint32_t)d[i + 2] << 16;
-    if (tail >= 2) k ^= (uint32_t)d[i + 1] << 8;
-    if (tail >= 1) {
-        k ^= (uint32_t)d[i];
-        k = rotl(k * C1, 15) * C2;
-        h ^= k;
-    }
-    h ^= (uint32_t)len;
-    h ^= h >> 16; h *= 0x85ebca6bu; h ^= h >> 13; h *= 0xc2b2ae35u; h ^= h >> 16;
-    return h;
-}
-}  // namespace
 
 template <int KIND>
 __global__ void __launch_bounds__(256) hash_tokens_kernel(const uint8_t *__restrict__ bytes, const int64_t *__restrict__ off,
@@ -68,7 +16,8 @@ __global__ void __launch_bounds__(256) hash_tokens_kernel(const uint8_t *__restr
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n_tok; t += stride) {
         const int64_t b0 = off[t], len = off[t + 1] - b0;
-        out[t] = KIND == DSK_HASH_XXH32 ? xxh32(bytes + b0, len, seed) : murmur3_32(bytes + b0, len, seed);
+        SpanReader rd{bytes + b0};
+        out[t] = hash32<KIND>(rd, len, seed);
     }
 }
 

@@ -4,23 +4,11 @@
 // datasketch/hashfunc.py:18-28: sha1_hash64(data) = struct.unpack("<Q", ...digest()[:8])[0]
 // SHA-1 per FIPS 180-4 (the algorithm lives in OpenSSL behind hashlib, not in the reference's tree;
 // parity is pinned against hashlib in tests/test_sha1_gpu.py).  thread <-> token; tokens are short
-// (one 64-byte block up to 55 bytes) so the kernel is latency/ALU-bound, not HBM-bound.
-#include "dsk_common.cuh"
+// (one 64-byte block up to 55 bytes) so the kernel is latency/ALU-bound, not HBM-bound.  The SHA-1 core is
+// sha1_lo_hi in hash_core.cuh, shared with the shingle kernels.
+#include "hash_core.cuh"
 
 namespace dsk {
-
-__device__ __forceinline__ uint32_t rotl32(uint32_t x, int n) { return __funnelshift_l(x, x, n); }
-
-// byte i of the padded message (length len, total padded length plen)
-__device__ __forceinline__ uint32_t padded_byte(const uint8_t *__restrict__ d, int64_t len, int64_t plen, int64_t i) {
-    if (i < len) return d[i];
-    if (i == len) return 0x80u;
-    if (i >= plen - 8) {
-        const uint64_t bits = (uint64_t)len * 8ull;
-        return (uint32_t)((bits >> (8 * (plen - 1 - i))) & 0xFFu);
-    }
-    return 0u;
-}
 
 __global__ void __launch_bounds__(256) sha1_tokens_kernel(const uint8_t *__restrict__ bytes,
                                                           const int64_t *__restrict__ off, int64_t n_tok,
@@ -28,38 +16,9 @@ __global__ void __launch_bounds__(256) sha1_tokens_kernel(const uint8_t *__restr
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n_tok; t += stride) {
         const int64_t b0 = off[t], len = off[t + 1] - b0;
-        const uint8_t *d = bytes + b0;
-        const int64_t plen = ((len + 8) / 64 + 1) * 64;
-        uint32_t h0 = 0x67452301u, h1 = 0xEFCDAB89u, h2 = 0x98BADCFEu, h3 = 0x10325476u, h4 = 0xC3D2E1F0u;
-        for (int64_t blk = 0; blk < plen; blk += 64) {
-            uint32_t w[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-                const int64_t p = blk + 4 * i;
-                w[i] = (padded_byte(d, len, plen, p) << 24) | (padded_byte(d, len, plen, p + 1) << 16) |
-                       (padded_byte(d, len, plen, p + 2) << 8) | padded_byte(d, len, plen, p + 3);
-            }
-            uint32_t a = h0, b = h1, c = h2, e = h4, dd = h3;
-#pragma unroll
-            for (int i = 0; i < 80; ++i) {
-                uint32_t wi;
-                if (i < 16) wi = w[i];
-                else {
-                    wi = rotl32(w[(i - 3) & 15] ^ w[(i - 8) & 15] ^ w[(i - 14) & 15] ^ w[i & 15], 1);
-                    w[i & 15] = wi;
-                }
-                uint32_t f, k;
-                if (i < 20) { f = (b & c) | (~b & dd); k = 0x5A827999u; }
-                else if (i < 40) { f = b ^ c ^ dd; k = 0x6ED9EBA1u; }
-                else if (i < 60) { f = (b & c) | (b & dd) | (c & dd); k = 0x8F1BBCDCu; }
-                else { f = b ^ c ^ dd; k = 0xCA62C1D6u; }
-                const uint32_t tmp = rotl32(a, 5) + f + e + k + wi;
-                e = dd; dd = c; c = rotl32(b, 30); b = a; a = tmp;
-            }
-            h0 += a; h1 += b; h2 += c; h3 += dd; h4 += e;
-        }
-        // digest bytes are h0 (big endian), h1, ...; the reference reads the first 4 / 8 bytes little-endian
-        const uint32_t lo = __byte_perm(h0, 0, 0x0123), hi = __byte_perm(h1, 0, 0x0123);
+        SpanReader rd{bytes + b0};
+        uint32_t lo, hi;
+        sha1_lo_hi(rd, len, &lo, &hi);
         if (out_is_u64) static_cast<uint64_t *>(out)[t] = ((uint64_t)hi << 32) | lo;
         else static_cast<uint32_t *>(out)[t] = lo;
     }

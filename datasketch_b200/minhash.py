@@ -251,6 +251,19 @@ class MinHash:
         if batch:
             yield from run(batch)
 
+    @classmethod
+    def bulk_text(cls, texts, n: int = 1, unit: str = "word", **minhash_kwargs) -> List["MinHash"]:
+        """One MinHash per raw text document: ``MinHash.bulk([shingles(t, n, unit) for t in texts], **minhash_kwargs)``
+        with the word / character n-gram shingles built, hashed and signed on the device (``shingle.signatures``).
+        ``texts`` is a sequence of ``str`` or bytes-like documents, or a ``(d_text, d_offsets)`` pair of CUDA tensors."""
+        from .shingle import signatures
+        proto = cls(**minhash_kwargs)
+        perms = np.ascontiguousarray(np.asarray(proto.permutations, dtype=np.uint64))
+        sig = signatures(texts, n, unit, seed=proto.seed, hashfunc=proto.hashfunc, permutations=perms)
+        if not proto.is_empty():
+            sig = np.minimum(sig, proto.hashvalues)
+        return [cls._from_row(proto, row.copy()) for row in sig]
+
     # -- pickling: only host state travels (cf. minhash.py:529-537) ---------------------------------
     def __getstate__(self):
         self._flush()

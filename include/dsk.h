@@ -571,6 +571,37 @@ DSK_API int dsk_sha1_tokens(const uint8_t *d_bytes, const int64_t *d_byte_offset
 DSK_API int dsk_hash_tokens(const uint8_t *d_bytes, const int64_t *d_byte_offsets, int64_t n_tokens, int kind,
                             uint32_t seed, uint32_t *d_out, void *stream);
 
+/* ---- raw UTF-8 text to word / character n-gram tokens (DESIGN.md §4m) -------------------------------------------------
+ * Replaces the user's shingling loop in front of MinHash.bulk; the reference has none and leaves it to the user.  Document
+ * i is d_text[d_doc_offsets[i] : d_doc_offsets[i+1]], read as UTF-8 on its own.  Its units are its words (unit
+ * DSK_SHINGLE_WORD: str.split() with no argument, i.e. maximal runs of code points outside Python's 29 whitespace code
+ * points) or its code points (DSK_SHINGLE_CHAR).  With m units it has max(m - n + 1, min(m, 1)) shingles: shingle j is
+ * units j .. j+n-1 (all m when m < n), words joined by one space, code points as they stand.  Each shingle becomes one
+ * 32-bit token, the token hash of its UTF-8 bytes, and the tokens of all documents, with d_tok_offsets, go unchanged to
+ * dsk_minhash_bulk_ws.  datasketch_b200/shingle.py:shingles() is the definition in Python.
+ * Every count and offset is int64 (the text may exceed 4 GiB); the work is spread over the bytes, not the documents.
+ *   dsk_shingle_workspace_size   bytes of the workspace both calls share: 16-byte aligned, owned by the caller, contents
+ *                                undefined on entry to dsk_shingle_count; 16 bytes per 2 KiB of text and 28 per document.
+ *   dsk_shingle_count  checks the offsets (non-decreasing, inside [0, n_bytes]) and the UTF-8 of every document as CPython's
+ *                      strict decoder does, and writes d_doc_status[n_docs + 1] (int32) and d_tok_offsets[n_docs + 1]
+ *                      (int64, the exclusive scan of the shingle counts; the total at [n_docs]).  d_doc_status[i] is 0 or
+ *                      DSK_SHINGLE_INVALID_UTF8, and such a document gets no shingles; d_doc_status[n_docs] is the OR of
+ *                      all of them, plus DSK_SHINGLE_BAD_OFFSETS when the offsets are malformed (then every count is 0 and
+ *                      no byte is read through them).  The caller reads the total and the summary back to size d_tokens.
+ *   dsk_shingle_hash   with the same text, offsets, unit, n and the workspace dsk_shingle_count filled: writes the token
+ *                      of shingle j of document i at d_tokens[d_tok_offsets[i] + j].  hash_kind: 0 = sha1_hash32, or
+ *                      DSK_HASH_XXH32 / DSK_HASH_MURMUR3_32 with `seed`. */
+#define DSK_SHINGLE_WORD 0
+#define DSK_SHINGLE_CHAR 1
+#define DSK_SHINGLE_INVALID_UTF8 1
+#define DSK_SHINGLE_BAD_OFFSETS 2
+DSK_API size_t dsk_shingle_workspace_size(int64_t n_docs, int64_t n_bytes);
+DSK_API int dsk_shingle_count(const uint8_t *d_text, const int64_t *d_doc_offsets, int64_t n_docs, int64_t n_bytes, int unit,
+                              int n, int64_t *d_tok_offsets, int32_t *d_doc_status, void *d_ws, size_t ws_bytes, void *stream);
+DSK_API int dsk_shingle_hash(const uint8_t *d_text, const int64_t *d_doc_offsets, int64_t n_docs, int64_t n_bytes, int unit,
+                             int n, int hash_kind, uint32_t seed, const int64_t *d_tok_offsets, uint32_t *d_tokens, void *d_ws,
+                             size_t ws_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
